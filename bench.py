@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the NeuralRecon-W per-ray training hot path on B200 (BASELINE.json metric).
+"""Benchmark of the NeuralRecon-W per-ray training hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl nrw|reference] [--precision bf16x3|bf16|bf16x6]
 
@@ -27,7 +27,7 @@ import torch.distributed as dist  # noqa: E402
 # algorithmic FLOP per sample (2*MAC, forward) of the three MLPs (SURVEY.md 8 / BASELINE.md 3)
 F_SDF, F_COL, F_NERF = 4195328, 1170688, 1318912
 DEFAULT_PRECISION = "mixed"      # headline precision policy: 3-product forward (outputs 1e-4), plain-bf16 backward GEMMs (DESIGN.md 6a;
-                                 # evidence: tests/test_gpu_precision_policy.py, profiles/r2_precision_study.json)
+                                 # evidence: tests/test_gpu_precision_policy.py)
 WORKLOADS = {
     "C3": dict(n_samples=64, n_importance=64, up_sample_steps=4, n_outside=4, rays=8192, fine=True, boundary_samples=10, sample_range=16,
                name="brandenburg_gate config + appearance embedding + surface-guided fine sampling (SDF-derived octree traced every step, "
@@ -51,7 +51,7 @@ def flop_per_ray(w):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md's clocks line), read
+    """SM clock and throttle reasons sampled DURING the timed region, read
     in-process through NVML every 100 ms.  (A looping `nvidia-smi --query-gpu` child was measured to stall kernel
     launches for seconds on boxes without persistence mode, so it is only the fallback, at a 1 s period.)"""
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -135,8 +135,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1409.5), d.get("hbm_gbs", 6576.7), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, sustained bf16)"
+    return 989.0, 3350.0, "fallback (H100 SXM data sheet: dense bf16 at 700 W, HBM3)"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -220,11 +220,11 @@ def torch_gpu_reference(workload, n_rays, steps, warmup, device):
 
 DTYPES = {"bf16": "bf16", "bf16x3": "bf16 (3-product split, fp32 accumulate)", "bf16x6": "bf16 (6-product split, fp32 accumulate)",
           "mixed": "bf16 (3-product split forward, plain bf16 backward, fp32 accumulate)"}
-NCU_TRAFFIC = os.path.join(ROOT, "profiles", "gemm_traffic.json")   # written from the round's `ncu --set full` capture
+NCU_TRAFFIC = os.path.join(ROOT, "profiles", "gemm_traffic.json")   # optional DRAM-traffic capture of the dominant launch (absent: traffic = null)
 
 
 def roofline_from_timing(L, out5, n_steps, ms_step, alg_flop_step, peak_tf, peak_src, workload=None):
-    """roofline of the dominant kernel family from the live CUDA-event timing of EVERY tcgen05 GEMM launch."""
+    """roofline of the dominant kernel family from the live CUDA-event timing of EVERY tensor-core GEMM launch."""
     k_ms, k_flop, k_mma, k_n, k_bytes = (out5[i] / n_steps for i in range(5))
     achieved = k_flop / (k_ms * 1e-3) / 1e12
     traffic = src = kernel = None
@@ -235,8 +235,8 @@ def roofline_from_timing(L, out5, n_steps, ms_step, alg_flop_step, peak_tf, peak
         kernel = t.get("kernel")
     return {"bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
             "traffic": traffic, "traffic_source": src, "peak_source": peak_src,
-            "kernel": "sdf_fused_kernel (fused forward-only SDF chain: encoding + 8 tcgen05 layers + head)" if workload == "C5" else
-                      "gemm_tc2_kernel / gemm_tc_kernel / sdf_fused_kernel (tcgen05 GEMM of every dense layer; the sampler's forward-only chains fused)",
+            "kernel": "sdf_fused_kernel (fused forward-only SDF chain: encoding + 8 wgmma layers + head)" if workload == "C5" else
+                      "gemm_tc_kernel / sdf_fused_kernel (wgmma GEMM of every dense layer; the sampler's forward-only chains fused)",
             "traffic_kernel": kernel,
             "launches_per_step": k_n, "kernel_ms_per_step": k_ms, "share_of_step": k_ms / ms_step,
             "algorithmic_tflop_per_step_in_kernel": k_flop / 1e12,
@@ -322,6 +322,8 @@ def bench_c5(args, rank, world, local):
     l0 = L.nrw_launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier(); e0.record(); vol = run(args.steps, False); e1.record(); barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"sdf": vol})
     launches = (L.nrw_launch_count() - l0) // max(args.steps, 1)
     ms = e0.elapsed_time(e1) / args.steps
     clk = clocks.stop() if rank == 0 else None
@@ -382,6 +384,28 @@ def bench_c5(args, rank, world, local):
         dist.destroy_process_group()
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays, seed=0):
+    """Writes what the timed path computed in its last step as out_dir/<name>.npy (float32, or float64 for float64 arrays),
+    so that two builds can be compared output for output.  An array larger than its share of the 64 MB budget is written as a
+    fixed, seeded sample of its flattened elements (<name>.npy) plus the sampled indices (<name>_index.npy, int64)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays)) - 4096      # bytes per array, .npy headers included
+    for name, t in arrays.items():
+        a = t.detach().cpu()
+        a = a.double() if a.dtype == torch.float64 else a.float()
+        a = a.numpy()
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(seed).choice(a.size, share // (a.itemsize + 8), replace=False)).astype(np.int64)
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx)
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 F_SDF_VALUE = 4195328 - 2 * 512 * 512     # value-only query: lin8 reduces to its sdf row (512 MACs), not 513 x 512
 
 
@@ -401,6 +425,8 @@ def main():
     ap.add_argument("--no_cpu_baseline", action="store_true")
     ap.add_argument("--no_torch_gpu_ref", action="store_true")
     ap.add_argument("--no_other_modes", action="store_true")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -505,13 +531,17 @@ def main():
     warm = max(args.warmup, 3)
     run(warm, False)
     ms, clk, launches, loss = timed(args.steps, False)
+    if args.dump_outputs and rank == 0:
+        eng = sysm.renderer.engine
+        dump_outputs(args.dump_outputs, {"loss": loss.double().reshape(1), "params": eng.flat, "grad": eng.last_flat_grad,
+                                         "embedding_a": sysm.embedding_a.weight})
     run(1, True)
     ms_e2e, clk2, _, _ = timed(args.steps, True)
     t = torch.tensor([ms, ms_e2e], device=device, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms, ms_e2e = float(t[0]), float(t[1])
-    # ---- roofline of the dominant kernel: CUDA events around EVERY tcgen05 GEMM launch of two more steps.
+    # ---- roofline of the dominant kernel: CUDA events around EVERY tensor-core GEMM launch of two more steps.
     # Every rank runs them (the step holds the gradient all-reduce); only rank 0's kernel times are reported. ----
     L.nrw_gemm_timing(1, None)
     sysm.stage_events = []

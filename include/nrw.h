@@ -1,4 +1,4 @@
-/* nrw.h - C ABI of the B200-native NeuralRecon-W per-ray training core (libnrw.so).
+/* nrw.h - C ABI of the H100-native NeuralRecon-W per-ray training core (libnrw.so).
  *
  * The reference (zju3dv/NeuralRecon-W) is pure Python: its seam for this path is the
  * duck-typed Python object NeuconWRenderer (rendering/renderer.py:51-961) plus the
@@ -38,7 +38,7 @@ typedef enum {
 
 typedef struct nrw_ctx nrw_ctx;
 
-/* GEMM backends: 0 = tcgen05 tensor cores (product path), 1 = fp32 CUDA cores (verification). */
+/* GEMM backends: 0 = wgmma tensor cores (product path; the name NRW_GEMM_TCGEN05 is historical), 1 = fp32 CUDA cores (verification). */
 #define NRW_GEMM_TCGEN05 0
 #define NRW_GEMM_SIMT 1
 
@@ -84,7 +84,7 @@ NRW_API int nrw_ctx_bind(nrw_ctx* ctx, void* packed, long long packed_bytes, voi
 NRW_API int nrw_pack_weights(nrw_ctx* ctx, const float* params, void* stream);
 
 /* ---- NeuconWRenderer.sdf / NeuconW.sdf  (rendering/renderer.py:947-949) -----------------
- * With two-plane operands on the tcgen05 backend the whole query is ONE launch of the fused on-chip chain (encoding, 8 layers,
+ * With two-plane operands on the tensor-core backend the whole query is ONE launch of the fused on-chip chain (encoding, 8 layers,
  * head; 12 B in / 4 B out of HBM per point) and touches no workspace; otherwise it runs chunk by chunk through the bound
  * workspace.  Results do not depend on how the caller batches the points. */
 NRW_API int nrw_sdf_query(nrw_ctx* ctx, const float* pts /*[n,3]*/, long long n, float* sdf /*[n]*/,
@@ -271,12 +271,12 @@ NRW_API int nrw_gemm_test(int backend, int n_planes, int mn_major, int k_slices,
                           const float* A, const float* B, const float* bias, int act, float* D,
                           void* scratch, void* stream);
 NRW_API long long nrw_launch_count(void);
-/* measurement: while enabled, every tcgen05 GEMM launch is bracketed by CUDA events on its stream; a call with
+/* measurement: while enabled, every tensor-core GEMM launch is bracketed by CUDA events on its stream; a call with
  * out5 != NULL synchronises those events and returns {sum of kernel ms, algorithmic FLOP (2MNK), MMA FLOP
  * (x plane products), launches, algorithmic HBM bytes (operands + epilogue streams)} since the last read
  * (bench.py roofline). */
 NRW_API int nrw_gemm_timing(int enable, double* out5_host);
-/* debug: per-CTA cycle attribution of the tcgen05 GEMM (u64 [SMs,16], zeroed by the caller; NULL = off) */
+/* debug: per-CTA cycle attribution of the tensor-core GEMM (u64 [SMs,16], zeroed by the caller; NULL = off) */
 NRW_API int nrw_debug_gemm_profile(void* device_buf_u64);
 
 #ifdef __cplusplus

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Build libnrw.so (sm_100a only) in-tree: neuralrecon-w_b200/nrw/libnrw.so
+# Build libnrw.so (sm_90a only) in-tree: neuralrecon-w_b200/nrw/libnrw.so
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"
 SRC="$HERE/csrc"
@@ -7,7 +7,7 @@ OUT="$HERE/nrw/libnrw.so"
 OBJ="$HERE/build"
 mkdir -p "$OBJ"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden --expt-relaxed-constexpr"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden --expt-relaxed-constexpr"
 pids=()
 for f in gemm_tc gemm_simt pack pointwise embed sampler composite octree octree_build optim dataio engine c_api; do
   if [ ! -f "$OBJ/$f.o" ] || [ "$SRC/$f.cu" -nt "$OBJ/$f.o" ] || [ -n "$(find "$SRC" "$HERE/../include" -name '*.h' -newer "$OBJ/$f.o" -o -name '*.cuh' -newer "$OBJ/$f.o" 2>/dev/null | head -1)" ]; then

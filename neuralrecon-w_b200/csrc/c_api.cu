@@ -359,8 +359,8 @@ int nrw_gemm_timing(int enable, double* out5 /* host: ms, algorithmic FLOP, MMA 
   return NRW_OK;
   NRW_GUARD_END
 }
-int nrw_debug_gemm_profile(void* device_buf_u64_148x8) {
-  gemm_tc_set_profile_buffer(reinterpret_cast<unsigned long long*>(device_buf_u64_148x8));
+int nrw_debug_gemm_profile(void* device_buf_u64_sms_x16) {
+  gemm_tc_set_profile_buffer(reinterpret_cast<unsigned long long*>(device_buf_u64_sms_x16));
   return NRW_OK;
 }
 

@@ -1,4 +1,4 @@
-// Common device/host helpers for the nrw CUDA library (sm_100a only).
+// Common device/host helpers for the nrw CUDA library (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>

@@ -23,8 +23,7 @@ __device__ __forceinline__ float pe4(const float* x, int j) {
 
 // ---- staged encoders -------------------------------------------------------------------------------------------------
 // A block of 128 threads owns ER = 32 consecutive rows.  Phase 1: one thread per (row, coordinate) evaluates sincosf ONCE per
-// frequency (the first version spent one sinf or cosf per OUTPUT element: the kernels were SFU/issue bound at 8-14 % of HBM
-// peak, profiles/r2_pointwise_ncu_summary.txt) and leaves the fp32 feature rows in shared memory.  Phase 2: all threads write
+// frequency (one sinf or cosf per OUTPUT element makes the kernel SFU / issue bound) and leaves the fp32 feature rows in shared memory.  Phase 2: all threads write
 // the bf16 planes with 4-byte bf16x2 stores, a warp per 128-byte row segment.
 static constexpr int ER = 32;
 

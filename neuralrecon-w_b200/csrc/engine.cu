@@ -1,6 +1,6 @@
 // Chunked orchestration of the per-ray hot path: sampler -> background NeRF -> SDF value/normal ->
 // colour net -> compositing, and the hand-derived backward of all of it (SURVEY.md 9.2/9.3).
-// Every dense layer is one tcgen05 GEMM launch with a fused epilogue; chunks of `Mc` samples keep the
+// Every dense layer is one tensor-core GEMM launch with a fused epilogue; chunks of `Mc` samples keep the
 // inter-layer activations L2-resident.  Backward recomputes the forward of a chunk into the workspace
 // and immediately consumes it, so memory is O(chunk) instead of O(batch).
 #include <stdlib.h>
@@ -167,10 +167,11 @@ static int mm_dw(nrw_ctx& c, Planes dY, Planes X, int M, int layer, cudaStream_t
   GemmDesc g;
   g.A = dY; g.B = X; g.n_planes = c.cur_planes;
   g.M = L.Np; g.N = L.Kp; g.K = M; g.mn_major = 1;
-  const int bn = (g.N <= 64) ? 64 : ((g.N <= 128 || c.cur_planes >= 3) ? 128 : 256);
-  const int tiles = cdiv(g.M, 128) * cdiv(g.N, bn);
-  int ks = 296 / tiles;
-  if (c.backend == NRW_GEMM_TCGEN05 && gemm_tc_wide_dw(g.M, g.N, c.cur_planes)) ks = 74 / (cdiv(g.M, 256) * cdiv(g.N, 512));   // one 256 x 512 tile per CTA pair
+  const int tiles = cdiv(g.M, 128) * cdiv(g.N, gemm_tc_tile_n(g.N));
+  int dev = 0, n_sm = 0;
+  NRW_CUDA_OK(cudaGetDevice(&dev));
+  NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+  int ks = 2 * n_sm / tiles;   // about two work items per SM
   const int max_ks = M / 512 > 0 ? M / 512 : 1;
   if (ks > max_ks) ks = max_ks;
   if (ks < 1) ks = 1;
@@ -200,7 +201,7 @@ static Planes rows(Planes P, int r0) { return Planes{P.p + (long long)r0 * P.ld,
 // forward chunks
 // ---------------------------------------------------------------------------------------------
 // A forward-only chain (encoding, 8 layers, head) runs as ONE kernel with the activations resident in shared memory
-// (gemm_tc.cu::sdf_fused_kernel); two-plane operands on the tcgen05 backend only (NRW_SDF_FUSED=0: per-layer launches).
+// (gemm_tc.cu::sdf_fused_kernel); two-plane operands on the tensor-core backend only (NRW_SDF_FUSED=0: per-layer launches).
 // It needs no chunk workspace.
 static bool sdf_fused_enabled(const nrw_ctx& c) {
   static const int fused_chain = getenv("NRW_SDF_FUSED") ? atoi(getenv("NRW_SDF_FUSED")) : 1;
@@ -222,7 +223,7 @@ int sdf_chunk_forward(nrw_ctx& c, int M, const float* pts, bool need_normal, boo
   const float* w0 = c.f_area + c.pm.heads.sdf_w0;
   const float* b0 = c.f_area + c.pm.heads.sdf_b0;
   // forward-only query (sampler, NeuconWRenderer.sdf, mesh / refresh pipelines): the SDF head is fused into the epilogue of
-  // the last layer - u_8 is never written, the head kernel never reads it (CTA-pair tcgen05 kernel only: M >= 256)
+  // the last layer - u_8 is never written, the head kernel never reads it (tensor-core kernel, M >= 256)
   static const int no_fused_head = getenv("NRW_FUSED_HEAD") ? !atoi(getenv("NRW_FUSED_HEAD")) : 0;
   const bool fused_head = !need_normal && !need_feat && M >= 256 && c.backend == NRW_GEMM_TCGEN05 && !no_fused_head;
   // NRW_SDF_FUSED=1: the whole forward-only chain (encoding, 8 layers, head) as ONE kernel with the activations resident in

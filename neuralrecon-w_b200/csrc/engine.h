@@ -6,7 +6,7 @@
 #include "params.h"
 #include "pointwise.h"
 
-// Forward activations of one chunk.  With enough HBM (180 GB on B200) every chunk of a training batch
+// Forward activations of one chunk.  With enough HBM every chunk of a training batch
 // keeps its own slot, so the backward pass consumes them directly instead of recomputing the forward.
 struct FwdSdfSlot {
   float* PTS;

@@ -1,4 +1,4 @@
-// Runtime-parameterised GEMM epilogue shared by the tcgen05 and SIMT GEMM kernels.
+// Runtime-parameterised GEMM epilogue shared by the tensor-core and SIMT GEMM kernels.
 //
 // For an accumulator element acc(m,n) of D = A * B^T the epilogue computes, in this order,
 //   v  = acc [+ bias[n]] [+ rowvec[m]*colvec[n]]
@@ -11,7 +11,7 @@
 // which covers every fused layer of the SDF / colour / background MLPs and their hand-derived
 // backward passes (DESIGN.md "GEMM call sites").  The arithmetic (epi_math) works on register arrays;
 // the two GEMM kernels differ only in how they move the aux inputs / outputs (direct per-row vectors
-// in the SIMT kernel, warp-transposed coalesced traffic through shared memory in the tcgen05 kernel).
+// in the SIMT kernel, warp-transposed coalesced traffic through shared memory in the tensor-core kernel).
 #pragma once
 #include "common.cuh"
 

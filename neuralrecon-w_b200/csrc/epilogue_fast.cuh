@@ -1,8 +1,8 @@
-// Compile-time specialised epilogues of the CTA-pair tcgen05 GEMM for the eight layer kinds that make up > 95 % of a
+// Compile-time specialised epilogues of the tensor-core GEMM for the eight layer kinds that make up > 95 % of a
 // training step.  Same arithmetic, in the same order, as the runtime-parameterised epi_chunk16 (epilogue_tc.cuh) - the
 // difference is what is NOT executed: ncu's source view of the generic epilogue showed ISETP + BRA + LOP3 + IMAD + LDC
 // (flag tests, alignment checks, 64-bit address arithmetic, ReLU bit masks) at > 50 % of all issued instructions and
-// the useful FADD / FMUL / F2FP at ~12 % (profiles/r2_gemm_epilogue_opmix.txt), with the backward layers of the
+// the useful FADD / FMUL / F2FP at ~12 % with the backward layers of the
 // `mixed` mode (one MMA product) bound by epilogue instruction issue, not by the tensor pipe or HBM.
 //
 // A kind is chosen on the host (pick_epi_kind) from the Epi descriptor; anything that does not match exactly, ragged
@@ -60,7 +60,7 @@ inline int pick_epi_kind(const Epi& e) {
   return EK_GENERIC;
 }
 
-// Side-stream loads of the epilogue.  The four epilogue warps of a TMEM lane quarter read NEIGHBOURING 64-byte (fp32) /
+// Side-stream loads of the epilogue.  Warps working on neighbouring column chunks of the same rows read NEIGHBOURING 64-byte (fp32) /
 // 32-byte (bf16) pieces of the same rows, so the first of them asks L2 to fetch the whole aligned 256 bytes
 // (ld.global.nc.L2::256B): the other three find their sectors in L2 instead of queueing a second HBM round trip.
 #ifndef NRW_EPI_L2_256B
@@ -119,15 +119,7 @@ __device__ __forceinline__ void line_colsum_add(const float (&w)[16], int lane, 
   }
 }
 
-// Prefetch schemes for the side streams, all measured by same-box A/B (profiles/r2e_epilogue_staging_ab.txt):
-//  * cp.async.bulk.prefetch.L2 of the next tile's streams one tile ahead: slower (102.5 vs 98.0 ms GEMM time per step), removed;
-//  * cp.async (LDGSTS, 8 bytes per lane) into lane-private shared-memory slots, double buffered: slower (reverse sweep
-//    343 -> 490 us), removed;
-//  * TMA boxes ([32 rows x 16 columns] bf16 per stream and chunk) into per-warp slots with per-warp mbarriers, issued by an
-//    elected lane (gemm_tc.cu): with 16 warps x 96 registers the extra state spills and it is slower; with 8 epilogue warps
-//    x 168 registers and a 3-deep queue it wins for GATE_FWD (480 -> 434 us) and loses for the one-product backward kinds
-//    (two warps per scheduler no longer hide the ALU chains) - kept, enabled for GATE_FWD only.
-// What did help: ld.global.nc.L2::256B on these loads (-1.2 % step time) and hoisting them above the transpose.
+// `sa` (optional): the chunk's side streams already staged in shared memory as [32 rows][16 columns] bf16 boxes.
 __device__ __forceinline__ bool epi_fast_eligible(const Epi& e, int m0w, int nc, int M, int N) {
   return M - m0w >= 32 && N - nc >= 16 && e.n_store - nc >= 16;
 }
@@ -202,8 +194,8 @@ __device__ __forceinline__ void epi_fast16(const Epi& e, float* stg, const float
     uint2 ru0[4];                     // first gate plane (further planes are loaded in place below, except GATE_FWD's second)
     float4 rf[4];                     // fp32 side stream (aux_q / aux_add), or its bf16 twin's raw bits in .x/.y;
                                       // GATE_FWD: raw bits of the SECOND gate plane in .x/.y (its own exposed round trip was
-                                      // 15 % of the stall samples, profiles/r2_gemm_fast_ncu.md); FWD_*: the bias in rf[0]
-    // `sa` != nullptr: the side streams of this chunk were brought into shared memory by TMA one chunk ahead (gemm_tc.cu):
+                                      // 15 % of the stall samples); FWD_*: the bias in rf[0]
+    // `sa` != nullptr: the side streams of this chunk are in shared memory:
     // stream 0 at sa, stream 1 at sa + 1024, each a row-major [32 rows][16 columns] bf16 box (32 bytes per row)
     const bool staged = sa != nullptr;
     if (staged) {

@@ -1,13 +1,12 @@
-// Epilogue of the tcgen05 GEMM kernels: one 32-row x 16-column chunk per call.
+// Epilogue of the tensor-core GEMM kernels: one 32-row x 16-column chunk per call.
 //
-// tcgen05.ld hands lane r of a warp ROW r of the accumulator (TMEM lane = row).  Doing the global I/O in
+// The GEMM hands lane r of a warp ROW r of the accumulator chunk (gemm_tc.cu stages it through shared memory).  Doing the global I/O in
 // that layout would touch 32 different cache lines per instruction, so the chunk is transposed ONCE
 // through a per-warp 2 KB shared staging tile (XOR-swizzled 16-byte slots, conflict-free both ways) into
 // the "line" layout: lane L owns columns 4*(L&3)..+3 of rows (L>>2) + 8*it, it = 0..3.  In that layout
 // every auxiliary load and every store of the epilogue is a direct, sector-aligned global access (8 rows
 // x 64 B per fp32 instruction, 8 rows x 32 B per bf16 instruction) and all arithmetic is elementwise, so
-// nothing else goes through shared memory.  16 epilogue warps (4 per TMEM lane quarter) keep four
-// independent chunks in flight per SM sub-partition; the chunk is small enough for 96 registers/thread.
+// nothing else goes through shared memory.
 #pragma once
 #include "epilogue.cuh"
 

@@ -16,7 +16,7 @@ struct GemmDesc {
 
 enum GemmBackend { GEMM_TCGEN05 = 0, GEMM_SIMT = 1 };
 
-// tcgen05 / TMEM / TMA implementation (gemm_tc.cu)
+// wgmma / TMA tensor-core implementation (gemm_tc.cu)
 int gemm_tc(const GemmDesc& g, cudaStream_t stream);
 // fp32 CUDA-core implementation over the same operands (gemm_simt.cu); verification backend
 int gemm_simt(const GemmDesc& g, cudaStream_t stream);
@@ -42,12 +42,11 @@ struct SdfFusedDesc {
 int sdf_fused_forward(const SdfFusedDesc& d, cudaStream_t stream);
 
 long long gemm_tc_launch_count();
-// true when gemm_tc runs this split-K weight-gradient shape (M x N output) on 256 x 512 pair tiles: the caller sizes k_slices for
-// one item per CTA pair
-bool gemm_tc_wide_dw(int M, int N, int n_planes);
-// debug: when non-null, every tcgen05 GEMM launch accumulates per-CTA cycle attribution into buf[148*8]
+// output columns of one gemm_tc tile (the caller of a split-K GEMM sizes k_slices from the tile count)
+inline int gemm_tc_tile_n(int N) { return N <= 64 ? 64 : 128; }
+// debug: when non-null, every tensor-core GEMM launch accumulates per-CTA cycle attribution into buf[SMs*16]
 void gemm_tc_set_profile_buffer(unsigned long long* buf);
-// measurement: CUDA events around every tcgen05 GEMM launch (on the launching stream)
+// measurement: CUDA events around every tensor-core GEMM launch (on the launching stream)
 void gemm_tc_timing_enable(bool on);
 int gemm_tc_timing_read(double* ms, double* flops, double* mma_flops, long long* launches, double* bytes);
 

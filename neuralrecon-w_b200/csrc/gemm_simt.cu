@@ -1,6 +1,6 @@
 // fp32 CUDA-core GEMM over the same split-bf16 operand planes and the same fused epilogue as
 // gemm_tc.cu.  It sums the planes back to fp32 (exact when 3 planes are used) and accumulates
-// with FFMA, so it is the in-library verification backend for the tcgen05 kernel and for the
+// with FFMA, so it is the in-library verification backend for the tensor-core kernel and for the
 // hand-derived backward passes.  It is still a CUDA path: nothing here runs on the host.
 #include "gemm.h"
 
@@ -72,7 +72,7 @@ int gemm_simt(const GemmDesc& g, cudaStream_t stream) {
   NRW_CHECK(g.M > 0 && g.N > 0 && g.K > 0, NRW_ERR_ARG, "gemm_simt: empty problem");
   NRW_CHECK(g.k_slices == 1 || g.epi.atomic, NRW_ERR_ARG, "gemm_simt: split-K needs an atomic epilogue");
   NRW_CHECK(!g.epi.out_pre_h && !g.epi.out2_h && !g.epi.aux_q_h && !g.epi.aux_add_h && !g.epi.head_w, NRW_ERR_ARG,
-            "gemm_simt: bf16 side streams are a tcgen05-path feature");
+            "gemm_simt: bf16 side streams are a tensor-core-path feature");
   dim3 grid(cdiv(g.N, TN), cdiv(g.M, TM), g.k_slices);
   if (g.mn_major)
     gemm_simt_kernel<1><<<grid, 256, 0, stream>>>(g.A, g.B, g.n_planes, g.M, g.N, g.K, g.k_slices, g.epi);

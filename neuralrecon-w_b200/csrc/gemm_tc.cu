@@ -1,18 +1,19 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a with split-bf16 operand planes and a fused epilogue.
+// wgmma / TMA GEMM for sm_90a (Hopper) with split-bf16 operand planes and a fused epilogue.
 //
-//   D[M,N] (fp32, TMEM) = sum_{(pa,pb) in products(n_planes)}  A_pa[M,K] * B_pb[N,K]^T
+//   D[M,N] (fp32, registers) = sum_{(pa,pb) in products(n_planes)}  A_pa[M,K] * B_pb[N,K]^T
 //
 // * operands are bf16 planes (hi / lo / lo2) of fp32 tensors; n_planes=1 is plain bf16,
 //   n_planes=2 issues hi*hi + hi*lo + lo*hi (~16 mantissa bits), n_planes=3 all six
 //   products whose weight is >= 2^-16 (~fp32).  All products accumulate into the same fp32
-//   TMEM accumulator, so precision is a loop bound, not a different kernel.
-// * persistent CTAs (one per SM), warp-specialised: warp 0 = TMA producer, warp 1 = MMA
-//   issuer (single elected thread, tcgen05.mma.cta_group::1.kind::f16, M=128, N=BN),
-//   warp 2 = TMEM allocator, warps 4.. = epilogue (tcgen05.ld 32x32b -> registers ->
-//   epi_apply -> global).  smem ring of TMA stages (128B swizzle), double-buffered TMEM
-//   accumulators so the epilogue of tile i overlaps the main loop of tile i+1.
+//   register accumulator, so precision is a loop bound, not a different kernel.
+// * persistent CTAs (one per SM), warp-specialised: warps 0-7 = two consumer warpgroups (each
+//   wgmma.m64nBNk16 on its 64 rows of the 128-row tile, then the epilogue of those rows), warp 8 =
+//   TMA producer.  smem ring of TMA stages (128B swizzle) so the loads of the next k-blocks (and of
+//   the next tile) overlap the MMAs and the epilogue.
+// * the epilogue stages a warpgroup's accumulators through shared memory into the row layout the
+//   chunk epilogues take (epilogue_tc.cuh / epilogue_fast.cuh: one 32-row x 16-column chunk per warp).
 // * mn_major=1 consumes both operands "transposed" straight from their natural row-major
-//   [rows=K][cols=M|N] layout (MN-major UMMA descriptors) - used for weight gradients
+//   [rows=K][cols=M|N] layout (MN-major wgmma descriptors) - used for weight gradients
 //   dW = dY^T X with split-K over the sample dimension and fp32 atomics in the epilogue.
 #include <stdlib.h>
 
@@ -28,18 +29,18 @@
 namespace nrw {
 
 static constexpr int BM = 128;
-static constexpr int BK = 64;            // 64 bf16 = 128 B = one swizzle row
-static constexpr int STAGE_BUDGET = 192 * 1024;
+static constexpr int BK = 64;                          // 64 bf16 = 128 B = one swizzle row
+static constexpr int RING_BYTES = 192 * 1024;          // TMA stages
 static constexpr int MAX_STAGES = 8;
-static constexpr int N_EPI_WARPS = 16;          // 4 per TMEM lane quarter, 16-column chunks (epilogue_tc.cuh)
-static constexpr int N_THREADS = 128 + 32 * N_EPI_WARPS;
-static constexpr int STG_BYTES = N_EPI_WARPS * 2048;   // per-warp 32x16 fp32 staging tiles (epilogue)
+static constexpr int N_CONSUMER_WARPS = 8;             // two warpgroups of 64 rows each
+static constexpr int N_THREADS = 32 * N_CONSUMER_WARPS + 32;
+static constexpr int EPI_LD = 36;                      // staging row pitch in floats: 32 columns + 4 (16-byte aligned rows)
+static constexpr int EPI_WG_BYTES = 64 * EPI_LD * 4;   // one warpgroup's staging tile [64 rows][32 columns]; doubles as 4 x 2 KB warp tiles
 static constexpr int CS_BYTES = 1024;                  // per-CTA column-sum accumulator (256 columns of one n-tile)
-static constexpr int BAR_BYTES = 512;                  // 20 pipeline mbarriers + TMEM pointer, then 32 side-stream mbarriers (CTA-pair kernel)
-static constexpr int AUX_SPLIT = 128 * 1024;           // side-stream staging on: operand ring [0, 128 KB), 16 x 2 x 2 KB slots [128 KB, 192 KB)
-static constexpr int AUX_SLOT_BYTES = 2048;
-static constexpr int SMEM_BYTES = 1024 + STAGE_BUDGET + BAR_BYTES + STG_BYTES + CS_BYTES;
-static_assert(SMEM_BYTES <= 232448, "dynamic shared memory limit of sm_100");
+static constexpr int BAR_BYTES = 256;                  // 2 x MAX_STAGES mbarriers
+static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + 2 * EPI_WG_BYTES + CS_BYTES;
+static_assert(SMEM_BYTES <= 232448, "dynamic shared memory limit of sm_90");
+static_assert(4 * 2048 <= EPI_WG_BYTES, "the 2 KB per-warp epilogue tiles live in the warpgroup's staging tile");
 
 struct TcParams {
   CUtensorMap tmA[3];
@@ -49,13 +50,10 @@ struct TcParams {
   int k_slices;
   int m_tiles, n_tiles;
   Epi epi;
-  // optional cycle attribution (debug): per CTA 8 counters
-  //  [0] producer: waiting for a free stage   [1] mma: waiting for TMA data   [2] mma: waiting for a free accumulator
-  //  [3] epilogue warp 4: waiting for the accumulator   [4] epilogue warp 4: busy   [5] kernel cycles   [6] tiles
+  // optional cycle attribution (debug): per CTA 16 counters
+  //  [0] producer: waiting for a free stage   [1] consumer warp 0: waiting for TMA data   [4] consumer warp 0: epilogue
+  //  [5] kernel cycles   [6] tiles
   unsigned long long* prof;
-  int dbg;   // tuning experiments (NRW_TC_DBG): bit0 = epilogue only drains TMEM, bit1 = one MMA per k-block
-  CUtensorMap tmX[2];   // CTA-pair kernel: bf16 side streams of the epilogue as [16 x 32] TMA boxes (no swizzle)
-  int aux_stage;        // stream mask (bit 0 / bit 1); 0 = the epilogue loads its side streams itself
 };
 #define NRW_PROF_T0(cond) const long long _t0 = (cond) ? clock64() : 0
 #define NRW_PROF_ADD(cond, slot) \
@@ -101,148 +99,129 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on the mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
 // Programmatic dependent launch: a GEMM launched with the stream-serialisation attribute may have its CTAs scheduled while the
-// previous kernel of the stream drains (each SM takes the next kernel's CTA as soon as its own finishes), so barrier init, TMEM
-// allocation and descriptor prefetch overlap the predecessor's tail.  pdl_wait() returns once the predecessor has completed and
-// its writes are visible: nothing before it may touch global memory.  Both are no-ops in a normally launched kernel.
+// previous kernel of the stream drains, so barrier init and descriptor prefetch overlap the predecessor's tail.  pdl_wait()
+// returns once the predecessor has completed and its writes are visible: nothing before it may touch global memory.  Both are
+// no-ops in a normally launched kernel.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-// one lane of the (converged) warp, the same one every time
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred P;\n"
-      "elect.sync _|P, 0xFFFFFFFF;\n"
-      "selp.u32 %0, 1, 0, P;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
+// named barrier over `n` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// generic-proxy shared-memory stores -> visible to the tensor core's (async proxy) reads
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// the same load without the wait: several may be in flight, tmem_ld_wait() before the first use of any of them
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, float (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]),
-        "=f"(v[8]), "=f"(v[9]), "=f"(v[10]), "=f"(v[11]), "=f"(v[12]), "=f"(v[13]), "=f"(v[14]), "=f"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory descriptor, 128B swizzle, version 1 (sm_100).
-//   bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// wgmma matrix descriptor (sm_90), 128B swizzle:
+//   bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 1 (128B swizzle)
+// K-major: SBO = 8 rows * 128 B (LBO unused).  MN-major: LBO = stride between 64-wide MN slabs, SBO = 8 k-rows * 128 B.
+__device__ __forceinline__ uint64_t make_gdesc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor for kind::f16: bf16 x bf16 -> fp32, M=128.
-__host__ __device__ constexpr uint32_t make_idesc(int n, int mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)mn_major << 15) | ((uint32_t)mn_major << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void acc_fence(float (&d)[N]) {   // keeps the accumulator registers in place across the async MMAs
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+
+// D[64 x BN] (+)= A[64 x 16] * B[BN x 16]^T, bf16 in, fp32 accumulate; TA / TB = 1: MN-major operand
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t da, uint64_t db, uint32_t accumulate);
+
+template <>
+__device__ __forceinline__ void wgmma_bf16<64, 0, 0>(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
+      "%26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<64, 1, 1>(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
+      "%26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+#define NRW_WGMMA_N128(TA, TB)                                                                                                          \
+  template <>                                                                                                                           \
+  __device__ __forceinline__ void wgmma_bf16<128, TA, TB>(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {              \
+    asm volatile(                                                                                                                       \
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"                                                                                    \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "                                                                        \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "    \
+        "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, " \
+        "%51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, " #TA ", " #TB ";\n}\n"                   \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),     \
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),        \
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),        \
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),        \
+          "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),        \
+          "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),        \
+          "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])         \
+        : "l"(da), "l"(db), "r"(accumulate));                                                                                           \
+  }
+NRW_WGMMA_N128(0, 0)
+NRW_WGMMA_N128(1, 1)
+#undef NRW_WGMMA_N128
 
 // product p of the plane expansion -> (a_plane, b_plane); ordered small-to-large magnitude last
 //   n_planes==1: (0,0); ==2: (0,1),(1,0),(0,0); ==3: (0,2),(2,0),(1,1),(0,1),(1,0),(0,0)
 // With q = n_products-1-p (q=0 is (hi,hi)): a_plane = nibble q of 0x021010, b_plane = nibble q of 0x201100.
 
-template <int BN, int MN_MAJOR>
+// EK: compile-time epilogue kind (epilogue_fast.cuh); MN-major launches use EK_GENERIC.
+template <int BN, int MN_MAJOR, int EK>
 __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
+  static_assert(BN == 64 || BN == 128, "wgmma tile width");
   constexpr int A_TILE = BM * BK * 2;
   constexpr int B_TILE = BN * BK * 2;
-  constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;  // two accumulator stages (power of 2)
+  constexpr int WG_A = 64 * BK * 2;           // one warpgroup's 64 rows of the A tile (K-major: 64 rows; MN-major: one 64-wide slab)
   extern __shared__ uint8_t smem_raw[];
   // align inside the shared window by OFFSET (an integer round trip of the pointer would turn every staging access
   // into a generic LD/ST instead of LDS/STS)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int P = p.n_planes;
   const int stage_bytes = P * (A_TILE + B_TILE);
-  int stages = STAGE_BUDGET / stage_bytes;
+  int stages = RING_BYTES / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGE_BUDGET);
-  // bars[0..8) full, [8..16) empty, [16..18) tmem_full, [18..20) tmem_empty; then tmem ptr
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 20);
-  const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + 8);
-  const uint32_t bar_tfull = smem_u32(bars + 16), bar_tempty = smem_u32(bars + 18);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
+  const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + MAX_STAGES);
+  float* epi_buf = reinterpret_cast<float*>(smem + RING_BYTES + BAR_BYTES);
+  float* cs_buf = reinterpret_cast<float*>(smem + RING_BYTES + BAR_BYTES + 2 * EPI_WG_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long t_kernel0 = clock64();
 
-  if (warp == 0 && lane == 0) {
+  if (warp == N_CONSUMER_WARPS && lane == 0) {
     for (int i = 0; i < P; ++i) {
       tma_prefetch_desc(&p.tmA[i]);
       tma_prefetch_desc(&p.tmB[i]);
     }
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < MAX_STAGES; ++i) {
       mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar_tfull + 8 * i, 1);
-      mbar_init(bar_tempty + 8 * i, N_EPI_WARPS);
+      mbar_init(bar_empty + 8 * i, N_CONSUMER_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) tmem_alloc(smem_u32(tmem_ptr_smem), TMEM_COLS);
-  float* cs_buf = reinterpret_cast<float*>(smem + STAGE_BUDGET + BAR_BYTES + STG_BYTES);
   if (threadIdx.x < 256) cs_buf[threadIdx.x] = 0.0f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
   pdl_launch_dependents();
 
@@ -251,7 +230,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
   const int n_items = p.m_tiles * p.n_tiles * p.k_slices;
   const int n_prod = (P == 1) ? 1 : (P == 2 ? 3 : 6);
 
-  if (warp == 0) {
+  if (warp == N_CONSUMER_WARPS) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int s = 0;
@@ -289,469 +268,116 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    {   // whole warp, one elected issuing lane (see the CTA-pair kernel below)
-      const bool issuer = elect_one();
-      const bool prof_m = p.prof != nullptr && lane == 0;
-      const uint32_t smem0 = smem_u32(smem);
-      constexpr uint32_t idesc = make_idesc(BN, MN_MAJOR);
-      // K-major: SBO = 8 rows * 128 B; MN-major: LBO = stride between 64-wide MN slabs, SBO = 8 k-rows
-      constexpr uint32_t LBO = MN_MAJOR ? (64 * BK * 2) : 16;
-      constexpr uint32_t SBO = 1024;
-      constexpr uint32_t KSTEP = MN_MAJOR ? (16 * 128) : 32;  // bytes per UMMA_K=16
-      int s = 0, acc = 0;
-      uint32_t ph = 0, acc_ph = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int ks = item % p.k_slices;
-        const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
-        {
-          NRW_PROF_T0(prof_m);
-          mbar_wait(bar_tempty + 8 * acc, acc_ph ^ 1);
-          NRW_PROF_ADD(prof_m, 2);
-        }
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        uint32_t accum = 0;
-        const uint64_t desc_hi = make_sdesc(0, LBO, SBO);   // everything but the start address
-        for (int kb = kb0; kb < kb1; ++kb) {
-          {
-            NRW_PROF_T0(prof_m);
-            mbar_wait(bar_full + 8 * s, ph);
-            NRW_PROF_ADD(prof_m, 1);
-          }
-          tc_fence_after();
-          const uint32_t sa = smem0 + s * stage_bytes;
-          const uint32_t sb = sa + P * A_TILE;
-          if (issuer) {
-            for (int pr = 0; pr < n_prod; ++pr) {
-              const int q = 4 * (n_prod - 1 - pr);           // product order of product_planes(), packed lookup
-              const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
-              const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE) & 0x3FFFFu) >> 4);
-              const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                umma_bf16(d_tmem, da + ((k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), idesc, accum);
-                accum = 1;
-              }
-            }
-            umma_commit(bar_empty + 8 * s);
-          }
-          __syncwarp();
-          if (++s == stages) { s = 0; ph ^= 1; }
-        }
-        // (an empty k-slice accumulates nothing but still hands the stage over so the roles stay in step)
-        if (issuer) umma_commit(bar_tfull + 8 * acc);
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int ew = warp - 4;
-    const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-    const int chalf = ew >> 2;                // column interleave among warps of the same quarter
-    constexpr int CH_PER = N_EPI_WARPS / 4;   // warps per quarter
-    float* stg = reinterpret_cast<float*>(smem + STAGE_BUDGET + BAR_BYTES) + ew * 512;
-    int acc = 0;
-    uint32_t acc_ph = 0;
+  } else {
+    // ===================== consumers: MMA, then the epilogue of the warpgroup's 64 rows =====================
+    const int wg = warp >> 2, wi = warp & 3;
+    const uint32_t smem0 = smem_u32(smem);
+    // K-major: SBO = 8 rows * 128 B; MN-major: LBO = stride between 64-wide MN slabs, SBO = 8 k-rows
+    constexpr uint32_t LBO = MN_MAJOR ? (64 * BK * 2) : 16;
+    constexpr uint32_t SBO = 1024;
+    constexpr uint32_t KSTEP = MN_MAJOR ? (16 * 128) : 32;  // bytes per wgmma K=16
+    const uint64_t desc_hi = make_gdesc(0, LBO, SBO);         // everything but the start address
+    float* stage_tile = epi_buf + wg * (EPI_WG_BYTES / 4);
+    float* stg = stage_tile + wi * 512;                      // this warp's 2 KB tile (after the staging tile has been read)
     const bool use_cs = p.epi.colsum != nullptr && !p.epi.atomic;
-    const int etid = threadIdx.x - 128;
+    const int ctid = threadIdx.x;
+    const bool prof = p.prof != nullptr && warp == 0 && lane == 0;
     int cs_n0 = -1;   // n-tile the shared column-sum accumulator currently holds
+    int s = 0;
+    uint32_t ph = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
       const int ks = item % p.k_slices;
       const int t = item / p.k_slices;
       const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * BM;
       const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
-      const bool prof = p.prof != nullptr && warp == 4 && lane == 0;
       if (use_cs && n0 != cs_n0) {
-        if (cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), etid, 32 * N_EPI_WARPS, 1);
+        if (cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 32 * N_CONSUMER_WARPS, 1);
         cs_n0 = n0;
       }
-      {
-        NRW_PROF_T0(prof);
-        mbar_wait(bar_tfull + 8 * acc, acc_ph);
-        NRW_PROF_ADD(prof, 3);
-      }
-      tc_fence_after();
-      {
-        NRW_PROF_T0(prof);
-        if (kb1 > kb0) {
-          for (int c = chalf; c < BN / 16; c += CH_PER) {
-            const int nc = n0 + c * 16;
-            if (nc >= p.N) break;               // warp-uniform
-            float v[16];
-            {
-              NRW_PROF_T0(prof);
-              tmem_ld16(tmem_base + acc * BN + c * 16 + ((uint32_t)(quarter * 32) << 16), v);
-              NRW_PROF_ADD(prof, 8);
-            }
-            epi_chunk16(p.epi, stg, v, m0 + quarter * 32, nc, p.M, p.N, lane, use_cs ? cs_buf + c * 16 : nullptr);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        NRW_PROF_ADD(prof, 4);
-        if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6], 1ull);
-      }
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-    }
-    if (use_cs && cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), etid, 32 * N_EPI_WARPS, 1);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (p.prof && threadIdx.x == 0) atomicAdd(&p.prof[blockIdx.x * 16 + 5], (unsigned long long)(clock64() - t_kernel0));
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// =======================================================================================
-// CTA-pair variant: tcgen05.mma.cta_group::2, one 256 x 256 tile per pair of SMs.
-//   Each CTA of the pair stages its own 128 rows of A and HALF of B (128 of the 256 weight rows); the
-//   leader CTA's single MMA thread issues M=256 instructions that read both CTAs' shared memory and
-//   write both CTAs' TMEM.  Per MMA-flop this halves the shared-memory operand reads and the L2->SMEM
-//   traffic of the 1-CTA kernel (which is shared-memory-bandwidth bound at N<=256).
-//   Barriers: full[s] lives on the leader and collects the TMA bytes of BOTH CTAs (.cta_group::2 loads
-//   with the peer bit of the mbarrier address cleared); empty[s] / tmem_full[] are signalled in both
-//   CTAs by multicast tcgen05.commit; tmem_empty[] on the leader collects both epilogues.
-// =======================================================================================
-static constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;   // clears the CTA-pair bit of a shared::cluster address
-static constexpr int BN2 = 256;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t bar_leader, int x, int y) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_leader), "r"(x), "r"(y)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {   // arrives on `bar` in BOTH CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"((unsigned short)3)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar & PEER_MASK) : "memory");
-}
-
-// NEW = number of epilogue warps (16, or 8 with more registers per thread and a 3-deep TMA prefetch of the side streams)
-// TN  = output columns per pair tile: 256 (two accumulator stages, the epilogue of one tile overlaps the MMAs of the next), or
-//       512 for the split-K weight-gradient GEMMs (MN-major operands, one item per pair): ONE 256 x 512 accumulator filling
-//       the TMEM, two N = 256 MMAs per K step that share the A tile, so a K block costs 48 KB of operand traffic per CTA
-//       instead of 2 x 32 KB.
-template <int MN_MAJOR, int EK, int NEW, int TN = 256>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(128 + 32 * NEW, 1) gemm_tc2_kernel(const __grid_constant__ TcParams p) {
-  static_assert(NEW == 16 || NEW == 8, "epilogue warps: 4 or 2 per TMEM lane quarter");
-  static_assert(TN == BN2 || (TN == 2 * BN2 && MN_MAJOR == 1 && EK == EK_GENERIC), "the 512-column tile exists for the weight-gradient GEMMs only");
-  constexpr int NBUF = NEW == 8 ? 4 : 2;           // 2 KB staging buffers per epilogue warp (<= 64 KB in total, 32 mbarriers)
-  constexpr int NMMA = TN / BN2;                   // N = 256 MMAs per K step
-  constexpr int NACC = 2 / NMMA;                   // accumulator stages in the 512 TMEM columns
-  constexpr int A_TILE = BM * BK * 2;              // this CTA's 128 rows of A
-  constexpr int B_SUB = (BN2 / 2) * BK * 2;        // this CTA's half of one MMA's B
-  constexpr int B_TILE = NMMA * B_SUB;
-  constexpr int TMEM_COLS = 2 * BN2;               // two 256-column accumulators, or one of 512
-  extern __shared__ uint8_t smem_raw[];
-  // align inside the shared window by OFFSET (an integer round trip of the pointer would turn every staging access
-  // into a generic LD/ST instead of LDS/STS)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int P = p.n_planes;
-  const int stage_bytes = P * (A_TILE + B_TILE);
-  const bool aux_on = NEW != 16 && EK != EK_GENERIC && MN_MAJOR == 0 && p.aux_stage != 0;   // staging lives in the 8-warp instantiations only
-  int stages = (aux_on ? AUX_SPLIT : STAGE_BUDGET) / stage_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGE_BUDGET);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 20);
-  const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + 8);
-  const uint32_t bar_tfull = smem_u32(bars + 16), bar_tempty = smem_u32(bars + 18);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < P; ++i) {
-      tma_prefetch_desc(&p.tmA[i]);
-      tma_prefetch_desc(&p.tmB[i]);
-    }
-    if (aux_on) {
-      tma_prefetch_desc(&p.tmX[0]);
-      if (p.aux_stage & 2) tma_prefetch_desc(&p.tmX[1]);
-    }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < MAX_STAGES; ++i) {
-      mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar_tfull + 8 * i, 1);
-      mbar_init(bar_tempty + 8 * i, 2 * NEW);
-    }
-    for (int i = 0; i < 32; ++i) mbar_init(smem_u32(bars + 32) + 8 * i, 1);   // side-stream slots: [warp][buffer]
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  float* cs_buf = reinterpret_cast<float*>(smem + STAGE_BUDGET + BAR_BYTES + STG_BYTES);
-  if (threadIdx.x < 256) cs_buf[threadIdx.x] = 0.0f;
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();
-  pdl_launch_dependents();
-
-  const int kb_total = (p.K + BK - 1) / BK;
-  const int kb_per = (kb_total + p.k_slices - 1) / p.k_slices;
-  const int n_items = p.m_tiles * p.n_tiles * p.k_slices;   // m_tiles counts 256-row tiles
-  const int n_prod = (P == 1) ? 1 : (P == 2 ? 3 : 6);
-  const int unit = blockIdx.x >> 1, n_units = gridDim.x >> 1;
-  const long long t_kernel0 = p.prof ? clock64() : 0;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    {   // whole warp walks the loop (uniform addresses), one elected lane issues
-      const bool issuer = elect_one();
-      const bool prof_p = p.prof != nullptr && lane == 0;
-      const uint32_t smem0 = smem_u32(smem);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int item = unit; item < n_items; item += n_units) {
-        const int ks = item % p.k_slices;
-        const int t = item / p.k_slices;
-        const int n0 = (t % p.n_tiles) * TN + (int)rank * (BN2 / 2);
-        const int m0 = (t / p.n_tiles) * (2 * BM) + (int)rank * BM;
-        const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          {
-            NRW_PROF_T0(prof_p);
-            mbar_wait(bar_empty + 8 * s, ph ^ 1);
-            NRW_PROF_ADD(prof_p, 0);
-          }
-          if (issuer) {
-            if (leader) mbar_arrive_expect_tx(bar_full + 8 * s, 2 * stage_bytes);
-            const uint32_t bfl = (bar_full + 8 * s) & PEER_MASK;
-            const uint32_t sa = smem0 + s * stage_bytes;
-            const uint32_t sb = sa + P * A_TILE;
-            for (int pl = 0; pl < P; ++pl) {
-              if (MN_MAJOR == 0) {
-                tma_load_2d_2sm(sa + pl * A_TILE, &p.tmA[pl], bfl, kb * BK, m0);
-                tma_load_2d_2sm(sb + pl * B_TILE, &p.tmB[pl], bfl, kb * BK, n0);
-              } else {
+      float acc[BN / 2];
 #pragma unroll
-                for (int sl = 0; sl < 2; ++sl) {
-                  tma_load_2d_2sm(sa + pl * A_TILE + sl * (64 * BK * 2), &p.tmA[pl], bfl, m0 + 64 * sl, kb * BK);
-#pragma unroll
-                  for (int j = 0; j < NMMA; ++j)      // MMA j covers columns [j * 256, +256) of the tile; this CTA holds its 128 of them
-                    tma_load_2d_2sm(sb + pl * B_TILE + j * B_SUB + sl * (64 * BK * 2), &p.tmB[pl], bfl, n0 + j * BN2 + 64 * sl, kb * BK);
-                }
-              }
-            }
-          }
-          __syncwarp();
-          if (++s == stages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    // The WHOLE warp walks the loop (warp-uniform control flow and addresses, so descriptors live in uniform
-    // registers) and one elected lane issues the tcgen05 instructions; a single-lane divergent region made the
-    // compiler wrap every MMA in a register->uniform-register "waterfall" loop and starved the issue slot.
-    if (leader) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)MN_MAJOR << 15) | ((uint32_t)MN_MAJOR << 16) |
-                                 ((uint32_t)(BN2 >> 3) << 17) | ((uint32_t)((2 * BM) >> 4) << 24);
-      constexpr uint32_t LBO = MN_MAJOR ? (64 * BK * 2) : 16;
-      constexpr uint32_t SBO = 1024;
-      constexpr uint32_t KSTEP = MN_MAJOR ? (16 * 128) : 32;
-      const uint64_t desc_hi = make_sdesc(0, LBO, SBO);          // everything but the start address
-      const uint32_t smem0 = smem_u32(smem);
-      const bool issuer = elect_one();
-      const bool prof_m = p.prof != nullptr && lane == 0;
-      int s = 0, acc = 0;
-      uint32_t ph = 0, acc_ph = 0;
-      for (int item = unit; item < n_items; item += n_units) {
-        const int ks = item % p.k_slices;
-        const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      int prev_s = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
         {
-          NRW_PROF_T0(prof_m);
-          mbar_wait(bar_tempty + 8 * acc, acc_ph ^ 1);
-          NRW_PROF_ADD(prof_m, 2);
+          NRW_PROF_T0(prof);
+          mbar_wait(bar_full + 8 * s, ph);
+          NRW_PROF_ADD(prof, 1);
         }
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN2;
-        uint32_t accum = 0;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          {
-            NRW_PROF_T0(prof_m);
-            mbar_wait(bar_full + 8 * s, ph);
-            NRW_PROF_ADD(prof_m, 1);
-          }
-          tc_fence_after();
-          const uint32_t sa = smem0 + s * stage_bytes;
-          const uint32_t sb = sa + P * A_TILE;
-          if (issuer) {
-            for (int pr = 0; pr < n_prod; ++pr) {
-              // product order: smallest magnitude first, (hi,hi) last; packed lookup (no local-memory tables)
-              const int q = 4 * (n_prod - 1 - pr);
-              const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
-              const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE) & 0x3FFFFu) >> 4);
-              const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
+        const uint32_t sa = smem0 + s * stage_bytes + wg * WG_A;
+        const uint32_t sb = smem0 + s * stage_bytes + P * A_TILE;
+        wgmma_fence();
+        for (int pr = 0; pr < n_prod; ++pr) {
+          const int q = 4 * (n_prod - 1 - pr);           // product order of product_planes(), packed lookup
+          const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
+          const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE) & 0x3FFFFu) >> 4);
+          const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
 #pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                if ((p.dbg & 2) && (pr | k)) continue;
-#pragma unroll
-                for (int j = 0; j < NMMA; ++j)
-                  umma_bf16_2sm(d_tmem + j * BN2, da + ((k * KSTEP) >> 4), db + ((j * B_SUB + k * KSTEP) >> 4), idesc, accum);
-                accum = 1;
-              }
-            }
-            umma_commit_2sm(bar_empty + 8 * s);
-          }
-          __syncwarp();
-          if (++s == stages) { s = 0; ph ^= 1; }
+          for (int k = 0; k < BK / 16; ++k)
+            wgmma_bf16<BN, MN_MAJOR, MN_MAJOR>(acc, da + ((k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
         }
-        if (issuer) umma_commit_2sm(bar_tfull + 8 * acc);
-        __syncwarp();
-        if (++acc == NACC) { acc = 0; acc_ph ^= 1; }
+        wgmma_commit();
+        acc_fence(acc);
+        if (prev_s >= 0) {                                // the previous stage's MMAs have completed: hand it back
+          wgmma_wait<1>();
+          acc_fence(acc);
+          if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+        }
+        prev_s = s;
+        if (++s == stages) { s = 0; ph ^= 1; }
       }
-    }
-  } else if (warp >= 4 && warp < 4 + NEW) {
-    // ===================== epilogue (both CTAs, own 128 rows) =====================
-    const int ew = warp - 4;
-    const int quarter = warp & 3;
-    const int chalf = ew >> 2;
-    constexpr int CH_PER = NEW / 4;
-    float* stg = reinterpret_cast<float*>(smem + STAGE_BUDGET + BAR_BYTES) + ew * 512;
-    int acc = 0;
-    uint32_t acc_ph = 0;
-    const bool use_cs = TN == BN2 && p.epi.colsum != nullptr && !p.epi.atomic;
-    const int etid = threadIdx.x - 128;
-    int cs_n0 = -1;   // n-tile the shared column-sum accumulator currently holds
-    // ---- side-stream staging: this warp's NBUF 2 KB slots + their mbarriers; a [32 x 16] bf16 TMA box per stream and
-    // chunk, issued NBUF-1 chunks ahead by one elected lane: deep asynchronous prefetch without registers.  The issue cursor
-    // (q_item, q_c) walks exactly the chunk sequence of the loops below. ----
-    const uint8_t* aux_gen = smem + AUX_SPLIT + ew * (NBUF * AUX_SLOT_BYTES);
-    const uint32_t aux_slot = smem_u32(aux_gen);
-    const uint32_t aux_bar = smem_u32(bars + 32) + 8 * NBUF * ew;
-    uint32_t aux_ph = 0, aux_issued = 0;          // per-buffer phase bits / "a load is in flight or landed" bits
-    int aux_k = 0, q_k = 0, q_item = unit, q_c = chalf;
-    auto aux_issue_next = [&]() {                 // issue the loads of the chunk under the cursor (if any), advance the cursor
-      while (q_item < n_items && (q_item % p.n_tiles) * BN2 + q_c * 16 >= p.N) { q_item += n_units; q_c = chalf; }   // tile without a chunk for this warp
-      if (q_item >= n_items) return;
-      const int im0w = (q_item / p.n_tiles) * (2 * BM) + (int)rank * BM + quarter * 32;
-      const int inc = (q_item % p.n_tiles) * BN2 + q_c * 16;
-      const int buf = q_k % NBUF;
-      const bool ok = epi_fast_eligible(p.epi, im0w, inc, p.M, p.N);
-      __syncwarp();                               // every lane has read the slot's previous contents
-      if (ok && elect_one()) {
-        const uint32_t bar = aux_bar + 8 * buf, dst = aux_slot + buf * AUX_SLOT_BYTES;
-        mbar_arrive_expect_tx(bar, (p.aux_stage & 2) ? 2048u : 1024u);
-        tma_load_2d(dst, &p.tmX[0], bar, inc, im0w);
-        if (p.aux_stage & 2) tma_load_2d(dst + 1024, &p.tmX[1], bar, inc, im0w);
-      }
-      __syncwarp();
-      aux_issued = ok ? (aux_issued | (1u << buf)) : (aux_issued & ~(1u << buf));
-      ++q_k;
-      q_c += CH_PER;
-      if (q_c >= BN2 / 16 || (q_item % p.n_tiles) * BN2 + q_c * 16 >= p.N) { q_item += n_units; q_c = chalf; }
-    };
-    if (aux_on) {
-#pragma unroll 1
-      for (int i = 0; i < NBUF - 1; ++i) aux_issue_next();
-    }
-    for (int item = unit; item < n_items; item += n_units) {
-      const int ks = item % p.k_slices;
-      const int t = item / p.k_slices;
-      const int n0 = (t % p.n_tiles) * TN;
-      const int m0 = (t / p.n_tiles) * (2 * BM) + (int)rank * BM;
-      const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
-      if (use_cs && n0 != cs_n0) {
-        if (cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN2), etid, 32 * NEW, 1);
-        cs_n0 = n0;
-      }
-      const bool prof = p.prof != nullptr && warp == 4 && lane == 0;
-      {
-        NRW_PROF_T0(prof);
-        mbar_wait(bar_tfull + 8 * acc, acc_ph);
-        NRW_PROF_ADD(prof, 3);
-      }
-      tc_fence_after();
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+      // (an empty k-slice accumulates nothing and stores nothing)
+      if (kb1 <= kb0) continue;
       NRW_PROF_T0(prof);
       if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6], 1ull);
+      // ---- epilogue: 32 columns at a time through the warpgroup's staging tile.  Fragment of warp wi: acc[4j + {0,1}] = row
+      // 16 wi + lane / 4, columns 8 j + 2 (lane % 4) + {0,1}; acc[4j + {2,3}] = the same columns of row + 8.  After the barrier warp
+      // wi takes rows 32 (wi & 1) .. +31 (row = lane) and columns 16 (wi >> 1) .. +15 of the 32: the chunk layout of epi_chunk16. ----
+      const int r0 = 16 * wi + (lane >> 2), c0 = 2 * (lane & 3);
+      const int qq = wi & 1, cc = wi >> 1;
+      const int m0w = m0 + 64 * wg + 32 * qq;
       float hacc[4] = {0.0f, 0.0f, 0.0f, 0.0f};     // FWD_HEAD: this lane's rows of the fused SDF-head dot product
-      if (kb1 > kb0) {
-        for (int c = chalf; c < TN / 16; c += CH_PER) {
-          const int nc = n0 + c * 16;
-          if (nc >= p.N) break;
-          const int m0w = m0 + quarter * 32;
-          const uint8_t* sa = nullptr;
-          if (aux_on) {
-            aux_issue_next();                                  // the chunk NBUF-1 ahead -> the buffer consumed last iteration
-            const int cur_buf = aux_k % NBUF;
-            if ((aux_issued >> cur_buf) & 1u) {
-              mbar_wait(aux_bar + 8 * cur_buf, (aux_ph >> cur_buf) & 1u);
-              aux_ph ^= 1u << cur_buf;
-              sa = aux_gen + cur_buf * AUX_SLOT_BYTES;
-            }
-            ++aux_k;
-          }
-          float v[16];
-          tmem_ld16(tmem_base + acc * BN2 + c * 16 + ((uint32_t)(quarter * 32) << 16), v);
-          if (!(p.dbg & 1)) epi_fast16<EK>(p.epi, stg, v, m0w, nc, p.M, p.N, lane, use_cs ? cs_buf + c * 16 : nullptr, sa, p.aux_stage, hacc);
-        }
-        if (EK == EK_FWD_HEAD && (lane & 3) == 0) {   // partial[row][slot], slot = n-tile * CH_PER + column class: plain stores
-          const int slot = (n0 / BN2) * CH_PER + chalf;
+      const int n_cp = (min(BN, p.N - n0) + 31) / 32;
 #pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int row = m0 + quarter * 32 + it * 8 + (lane >> 2);
-            if (row < p.M) p.epi.head_partial[(long long)row * 8 + slot] = hacc[it];
-          }
+      for (int cp = 0; cp < BN / 32; ++cp) {
+        if (cp >= n_cp) break;                       // warpgroup-uniform
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = 4 * cp + jj;
+          *reinterpret_cast<float2*>(stage_tile + r0 * EPI_LD + 8 * jj + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(stage_tile + (r0 + 8) * EPI_LD + 8 * jj + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        named_bar_sync(2 + wg, 128);
+        float v[16];
+        const float* src = stage_tile + (32 * qq + lane) * EPI_LD + 16 * cc;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float4 t4 = *reinterpret_cast<const float4*>(src + 4 * i);
+          v[4 * i] = t4.x; v[4 * i + 1] = t4.y; v[4 * i + 2] = t4.z; v[4 * i + 3] = t4.w;
+        }
+        named_bar_sync(2 + wg, 128);                 // the staging tile is free: it holds the warps' 2 KB tiles from here on
+        const int nc = n0 + 32 * cp + 16 * cc;
+        if (nc < p.N && m0w < p.M)                   // warp-uniform
+          epi_fast16<EK>(p.epi, stg, v, m0w, nc, p.M, p.N, lane, use_cs ? cs_buf + 32 * cp + 16 * cc : nullptr, nullptr, 0, hacc);
+        named_bar_sync(2 + wg, 128);
+      }
+      if (EK == EK_FWD_HEAD && (lane & 3) == 0) {   // partial[row][slot], slot = n-tile * 2 + column class: plain stores
+        const int slot = (n0 / BN) * 2 + cc;
+#pragma unroll
+        for (int it = 0; it < 4; ++it) {
+          const int row = m0w + it * 8 + (lane >> 2);
+          if (row < p.M) p.epi.head_partial[(long long)row * 8 + slot] = hacc[it];
         }
       }
-      tc_fence_before();
-      __syncwarp();
       NRW_PROF_ADD(prof, 4);
-      if (lane == 0) mbar_arrive_leader(bar_tempty + 8 * acc);
-      if (++acc == NACC) { acc = 0; acc_ph ^= 1; }
     }
-    if (use_cs && cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN2), etid, 32 * NEW, 1);
+    if (use_cs && cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 32 * N_CONSUMER_WARPS, 1);
   }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();   // the peer may still signal our barriers / read our shared memory until here
   if (p.prof && threadIdx.x == 0) atomicAdd(&p.prof[blockIdx.x * 16 + 5], (unsigned long long)(clock64() - t_kernel0));
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS) : "memory");
-  }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -854,39 +480,19 @@ static cudaError_t launch_gemm(Kernel kernel, int grid, int block, cudaStream_t 
   return cudaLaunchKernelEx(&cfg, kernel, p);
 }
 
-template <int BN, int MN>
-static int launch(const TcParams& p, int n_sm, cudaStream_t stream) {
+template <int BN, int MN, int EK>
+static int launch(const TcParams& p, int n_sm, int dev, cudaStream_t stream) {
   static bool attr_set[MAX_DEV] = {false};
-  const int dev = current_device();
   if (!attr_set[dev]) {
-    NRW_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, MN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    NRW_CUDA_OK((cudaFuncSetAttribute(gemm_tc_kernel<BN, MN, EK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)));
     attr_set[dev] = true;
   }
   const int items = p.m_tiles * p.n_tiles * p.k_slices;
   const int grid = items < n_sm ? items : n_sm;
-  NRW_CUDA_OK(launch_gemm(gemm_tc_kernel<BN, MN>, grid, N_THREADS, stream, p));
+  NRW_CUDA_OK((launch_gemm(gemm_tc_kernel<BN, MN, EK>, grid, N_THREADS, stream, p)));
   NRW_LAUNCH_OK();
   ++g_tc_launches;
   return NRW_OK;
-}
-
-template <int MN, int EK, int NEW = N_EPI_WARPS, int TN = 256>
-static int launch2(const TcParams& p, int pairs, int dev, cudaStream_t stream) {
-  static bool attr_set[MAX_DEV] = {false};
-  if (!attr_set[dev]) {
-    NRW_CUDA_OK((cudaFuncSetAttribute(gemm_tc2_kernel<MN, EK, NEW, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)));
-    attr_set[dev] = true;
-  }
-  NRW_CUDA_OK((launch_gemm(gemm_tc2_kernel<MN, EK, NEW, TN>, 2 * pairs, 128 + 32 * NEW, stream, p)));
-  return NRW_OK;
-}
-
-// 512-column pair tiles for the split-K weight-gradient GEMMs (see gemm_tc2_kernel).  NRW_DW_WIDE: 0 off, 1 one-plane
-// operands only (default: two planes leave 2 TMA stages of 96 KB), 2 always.
-bool gemm_tc_wide_dw(int M, int N, int n_planes) {
-  static const int mode = getenv("NRW_DW_WIDE") ? atoi(getenv("NRW_DW_WIDE")) : 1;
-  static const int use_2cta = getenv("NRW_TC_2CTA") ? atoi(getenv("NRW_TC_2CTA")) : 1;
-  return use_2cta && mode > 0 && M >= 256 && N >= 2 * BN2 && n_planes <= (mode >= 2 ? 2 : 1);
 }
 
 static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream);
@@ -946,7 +552,6 @@ int gemm_tc(const GemmDesc& g, cudaStream_t stream) {
   g_timed.push_back(L);
   return rc;
 }
-
 static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
   NRW_CHECK(g.M > 0 && g.N > 0 && g.K > 0, NRW_ERR_ARG, "gemm_tc: empty problem %d %d %d", g.M, g.N, g.K);
   NRW_CHECK(g.n_planes >= 1 && g.n_planes <= 3, NRW_ERR_ARG, "gemm_tc: n_planes=%d", g.n_planes);
@@ -955,90 +560,14 @@ static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
   const int dev = current_device();
   if (!n_sm_dev[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm_dev[dev], cudaDevAttrMultiProcessorCount, dev));
   const int n_sm = n_sm_dev[dev];
-  int BN;
-  static const int bn_pref = getenv("NRW_TC_BN") ? atoi(getenv("NRW_TC_BN")) : 0;   // tuning override
-  if (g.N <= 64) BN = 64;
-  else if (g.N <= 128 || g.n_planes >= 3) BN = 128;
-  else if (g.n_planes == 2) BN = (bn_pref == 128) ? 128 : 256;   // 2 TMA stages of 96 KB, N=256 MMAs
-  else BN = (bn_pref == 128) ? 128 : 256;
+  // 128 x 128 tiles (two m64n128 warpgroups): with two operand planes that is 64 KB per k-block and 3 TMA stages
+  const int BN = g.N <= 64 ? 64 : 128;
   TcParams p;
   memset(&p, 0, sizeof(p));
   p.M = g.M; p.N = g.N; p.K = g.K; p.n_planes = g.n_planes; p.k_slices = g.k_slices;
   p.m_tiles = cdiv(g.M, BM); p.n_tiles = cdiv(g.N, BN);
   p.epi = g.epi;
   p.prof = g_prof_ptr;
-  static const int dbg = getenv("NRW_TC_DBG") ? atoi(getenv("NRW_TC_DBG")) : 0;
-  p.dbg = dbg;
-  // CTA-pair kernel (tcgen05 cta_group::2, 256 x 256 tiles) for the wide layers
-  static const int use_2cta = getenv("NRW_TC_2CTA") ? atoi(getenv("NRW_TC_2CTA")) : 1;
-  // NRW_PAIR_MIN_N: narrowest K-major layer that takes the CTA-pair kernel and its specialised epilogues (a 128-wide layer fills half
-  // of the 256-column pair tile: the second CTA's half of B is out of range and arrives as zeros)
-  static const int pair_min_n = getenv("NRW_PAIR_MIN_N") ? atoi(getenv("NRW_PAIR_MIN_N")) : 128;
-  if (use_2cta && g.M >= 256 && g.N >= (g.mn_major ? 256 : pair_min_n)) {
-    const bool wide = g.mn_major && g.epi.atomic && gemm_tc_wide_dw(g.M, g.N, g.n_planes);
-    p.m_tiles = cdiv(g.M, 2 * BM); p.n_tiles = cdiv(g.N, wide ? 2 * BN2 : BN2);
-    for (int pl = 0; pl < g.n_planes; ++pl) {
-      if (!g.mn_major) {
-        NRW_CHECK(g.K % BK == 0, NRW_ERR_ARG, "gemm_tc: K=%d must be a multiple of %d (pad the operand)", g.K, BK);
-        NRW_TRY(make_map(&p.tmA[pl], g.A.plane(pl), g.K, g.M, g.A.ld, BK, BM));
-        NRW_TRY(make_map(&p.tmB[pl], g.B.plane(pl), g.K, g.N, g.B.ld, BK, BN2 / 2));
-      } else {
-        NRW_TRY(make_map(&p.tmA[pl], g.A.plane(pl), g.M, g.K, g.A.ld, 64, BK));
-        NRW_TRY(make_map(&p.tmB[pl], g.B.plane(pl), g.N, g.K, g.B.ld, 64, BK));
-      }
-    }
-    const int items = p.m_tiles * p.n_tiles * p.k_slices;
-    int pairs = n_sm / 2;
-    if (items < pairs) pairs = items;
-    static const int use_fast = getenv("NRW_EPI_FAST") ? atoi(getenv("NRW_EPI_FAST")) : 1;   // 0: generic epilogue everywhere
-    const int ek = (g.mn_major || (!use_fast && !g.epi.head_w)) ? EK_GENERIC : pick_epi_kind(g.epi);
-    NRW_CHECK(ek >= 0 && (ek != EK_FWD_HEAD || (g.N == 2 * BN2 && N_EPI_WARPS == 16)), NRW_ERR_ARG,
-              "gemm_tc: the fused SDF-head epilogue needs N = 512, bias + softplus and no other output");
-    // side-stream staging by TMA: needs >= 2 operand stages in the remaining 128 KB, no split-K, and a stream set of the kind
-    // that fits 2 KB per chunk.  NRW_AUX_STAGE = per-kind bit mask (bit EK_*) for A/B runs.
-    // Measured per kind on one box (profiles/r2e_epilogue_staging_ab.txt): staging + 8 warps wins for the gradient-chain
-    // forward (3 MMA products, two gate planes: 480 -> 434 us per launch) and loses for the one-product backward kinds
-    // (reverse 343 -> 368 us, ReLU backward 140 -> 173 us), so the default stages GATE_FWD only.
-    static const int aux_kinds = getenv("NRW_AUX_STAGE") ? atoi(getenv("NRW_AUX_STAGE")) : (1 << EK_GATE_FWD);
-    p.aux_stage = 0;
-    if (ek != EK_GENERIC && g.k_slices == 1 && 2 * g.n_planes * (BM * BK * 2 + (BN2 / 2) * BK * 2) <= AUX_SPLIT && ((aux_kinds >> ek) & 1)) {
-      const bf16 *x0, *x1;
-      int ld0, ld1;
-      const int mask = pick_aux_streams(g.epi, ek, &x0, &ld0, &x1, &ld1);
-      if (mask && (ld0 % 8) == 0 && (!(mask & 2) || (ld1 % 8) == 0)) {
-        NRW_TRY(make_map(&p.tmX[0], x0, ld0, g.M, ld0, 16, 32, false));
-        if (mask & 2) NRW_TRY(make_map(&p.tmX[1], x1, ld1, g.M, ld1, 16, 32, false));
-        p.aux_stage = mask;
-      }
-    }
-    if (g.mn_major && wide) { NRW_TRY((launch2<1, EK_GENERIC, N_EPI_WARPS, 2 * BN2>(p, pairs, dev, stream))); }
-    else if (g.mn_major) { NRW_TRY((launch2<1, EK_GENERIC>(p, pairs, dev, stream))); }
-    else {
-      switch (ek) {
-        case EK_FWD_SOFTPLUS: NRW_TRY((launch2<0, EK_FWD_SOFTPLUS>(p, pairs, dev, stream))); break;
-        case EK_FWD_RELU: NRW_TRY((launch2<0, EK_FWD_RELU>(p, pairs, dev, stream))); break;
-        case EK_FWD_NONE: NRW_TRY((launch2<0, EK_FWD_NONE>(p, pairs, dev, stream))); break;
-        case EK_FWD_HEAD: NRW_TRY((launch2<0, EK_FWD_HEAD>(p, pairs, dev, stream))); break;
-        // staged side streams: 8 epilogue warps (168 registers, 3-deep TMA prefetch); otherwise 16 warps with register loads.
-        // (A 12-warp / 128-register / 1-deep variant was measured as well: no different, profiles/r2e_epilogue_staging_ab.txt.)
-#define NRW_STAGED_CASE(KIND)                                                            \
-  case KIND:                                                                             \
-    if (p.aux_stage) { NRW_TRY((launch2<0, KIND, 8>(p, pairs, dev, stream))); }          \
-    else { NRW_TRY((launch2<0, KIND>(p, pairs, dev, stream))); }                         \
-    break;
-        NRW_STAGED_CASE(EK_GATE_FWD)
-        NRW_STAGED_CASE(EK_TANGENT)
-        NRW_STAGED_CASE(EK_REVERSE)
-        NRW_STAGED_CASE(EK_RELU_BWD)
-#undef NRW_STAGED_CASE
-        default: NRW_TRY((launch2<0, EK_GENERIC>(p, pairs, dev, stream)));
-      }
-    }
-    NRW_LAUNCH_OK();
-    ++g_tc_launches;
-    return NRW_OK;
-  }
-  NRW_CHECK(!g.epi.head_w && !g.epi.head_partial, NRW_ERR_ARG, "gemm_tc: the fused SDF-head epilogue exists in the CTA-pair kernel only (M >= 256, N = 512)");
   for (int pl = 0; pl < g.n_planes; ++pl) {
     if (!g.mn_major) {
       NRW_CHECK(g.K % BK == 0, NRW_ERR_ARG, "gemm_tc: K=%d must be a multiple of %d (pad the operand)", g.K, BK);
@@ -1049,14 +578,22 @@ static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
       NRW_TRY(make_map(&p.tmB[pl], g.B.plane(pl), g.N, g.K, g.B.ld, 64, BK));
     }
   }
-  if (!g.mn_major) {
-    if (BN == 64) return launch<64, 0>(p, n_sm, stream);
-    if (BN == 128) return launch<128, 0>(p, n_sm, stream);
-    return launch<256, 0>(p, n_sm, stream);
-  } else {
-    if (BN == 64) return launch<64, 1>(p, n_sm, stream);
-    if (BN == 128) return launch<128, 1>(p, n_sm, stream);
-    return launch<256, 1>(p, n_sm, stream);
+  static const int use_fast = getenv("NRW_EPI_FAST") ? atoi(getenv("NRW_EPI_FAST")) : 1;   // 0: generic epilogue everywhere
+  const int ek = (g.mn_major || (!use_fast && !g.epi.head_w)) ? EK_GENERIC : pick_epi_kind(g.epi);
+  NRW_CHECK(ek >= 0 && (ek != EK_FWD_HEAD || g.N == 512), NRW_ERR_ARG,
+            "gemm_tc: the fused SDF-head epilogue needs N = 512, bias + softplus and no other output");
+  if (g.mn_major) return BN == 64 ? launch<64, 1, EK_GENERIC>(p, n_sm, dev, stream) : launch<128, 1, EK_GENERIC>(p, n_sm, dev, stream);
+  if (BN == 64) return launch<64, 0, EK_GENERIC>(p, n_sm, dev, stream);
+  switch (ek) {
+    case EK_FWD_SOFTPLUS: return launch<128, 0, EK_FWD_SOFTPLUS>(p, n_sm, dev, stream);
+    case EK_FWD_RELU: return launch<128, 0, EK_FWD_RELU>(p, n_sm, dev, stream);
+    case EK_FWD_NONE: return launch<128, 0, EK_FWD_NONE>(p, n_sm, dev, stream);
+    case EK_FWD_HEAD: return launch<128, 0, EK_FWD_HEAD>(p, n_sm, dev, stream);
+    case EK_GATE_FWD: return launch<128, 0, EK_GATE_FWD>(p, n_sm, dev, stream);
+    case EK_TANGENT: return launch<128, 0, EK_TANGENT>(p, n_sm, dev, stream);
+    case EK_REVERSE: return launch<128, 0, EK_REVERSE>(p, n_sm, dev, stream);
+    case EK_RELU_BWD: return launch<128, 0, EK_RELU_BWD>(p, n_sm, dev, stream);
+    default: return launch<128, 0, EK_GENERIC>(p, n_sm, dev, stream);
   }
 }
 
@@ -1066,48 +603,38 @@ static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
 //   positional encoding -> 8 x (512-wide layer, bias, softplus, [skip concat]) -> sdf head, ONE persistent kernel.
 //   models/neuconw.py:263-279 (SDFNetwork.forward) + :281-282 (sdf): the reference runs 9 Linear + 8 Softplus + cat per chunk.
 //
-//   A CTA pair owns 128 sample rows, 64 per CTA (tcgen05.mma.cta_group::2 with M = 128: each SM feeds 64 rows and half of the
-//   256 weight rows of an MMA; 64 rows x 256 columns of fp32 land in 128 lanes x 128 columns of its TMEM).  The two bf16 planes
-//   of the 64 x 512 activation tile live in shared memory (128 KB) in exactly the K-major 128B-swizzled layout the next layer's
-//   MMAs read; the weights stream from L2 through a 3-stage TMA ring (one stage = one 64-wide k-block of one 256-column half,
-//   both planes: 32 KB per CTA); accumulators ping-pong between the two halves of the TMEM by layer parity.  HBM sees 12 bytes
-//   per sample in and 4 bytes out.
-//
-//   Within a layer the MMA units (one unit = one k-block of one column half h, 12 instructions) are issued as
-//   [k-blocks 0-3, both halves], h0[k-blocks 4-7] -> commit, h1[k-blocks 4-7] -> commit (fz_unit_packed): once half 0 is
-//   committed every read of input k-blocks 0-3 has completed, so the epilogue of half 0 may overwrite them IN PLACE with the new
-//   activations (columns 0-255 of the output = k-blocks 0-3 of the next layer) while the tensor pipe still works on half 1; half 1
-//   then overwrites k-blocks 4-7.  Hand-over is per k-block: a_ready[kb] collects the 8 epilogue warps per CTA (both CTAs) that
-//   write k-block kb, and the next layer walks the k-blocks in the order the epilogue finishes them (0, 2, 1, 3 / 4, 6, 5, 7).
-//   Same product order per k-block as the per-layer kernels; the k-block order differs, so results agree with the per-layer
-//   chain to fp32 accumulation order (measured 4e-6), and are run-to-run bit-identical.
+//   A CTA owns 64 sample rows.  The two bf16 planes of the 64 x 512 activation tile live in shared memory (128 KB) in exactly
+//   the K-major 128B-swizzled layout the next layer's wgmma reads.  Four consumer warpgroups each compute 128 of the 512 output
+//   columns (two m64n64 register accumulators) over all k-blocks, and streams its own weights from L2 through a private 3-stage
+//   TMA ring (one stage = one 64-wide k-block of 64 weight rows, one plane: 8 KB): one thread of the warpgroup refills a stage
+//   as soon as the warpgroup's MMAs on it have completed, two stages ahead, across layer and tile boundaries.  Private rings keep
+//   every stage with a single consumer (no empty barriers, no producer warp: 512 threads leave 128 registers per thread).  Per k-block and 64-column half
+//   the lo-plane weights come first - product (hi, lo) - then the hi plane - (lo, hi), (hi, hi): the product order of the
+//   per-layer kernels.  Once every warpgroup has finished a layer's MMAs (named barrier) the epilogues overwrite the input
+//   activations IN PLACE with the new ones.  HBM sees 12 bytes per sample in and 4 bytes out.  Results agree with the
+//   per-layer chain to fp32 accumulation order and are run-to-run bit-identical (fixed-order head reduction).
 // =======================================================================================
 static constexpr int FZ_ROWS = 64;                         // rows per CTA
 static constexpr int FZ_APLANE = FZ_ROWS * 512 * 2;        // one bf16 plane of the activation tile: 8 k-blocks of [64 x 64]
 static constexpr int FZ_A = 2 * FZ_APLANE;
-static constexpr int FZ_WPL = 128 * BK * 2;                // this CTA's 128 weight rows of one k-block, one plane
-static constexpr int FZ_WSTAGE = 2 * FZ_WPL;
-static constexpr int FZ_NST = 3;
-static constexpr int FZ_BAR = FZ_A + FZ_NST * FZ_WSTAGE;
+static constexpr int FZ_WG = 4;                            // consumer warpgroups, 128 output columns each
+static constexpr int FZ_WSTAGE = 64 * BK * 2;              // 64 weight rows of one k-block, one plane
+static constexpr int FZ_NST = 3;                           // stages per warpgroup ring
+static constexpr int FZ_BAR = FZ_A + FZ_WG * FZ_NST * FZ_WSTAGE;
 static constexpr int FZ_SMEM = 1024 + FZ_BAR + 256;
-static constexpr int FZ_PART = 2 * 8192;                   // head partials [64 rows][16 slots] fp32 in k-block 2 of plane 0 (free by then)
-static_assert(FZ_SMEM <= 232448, "dynamic shared memory limit of sm_100");
+static constexpr int FZ_THREADS = 128 * FZ_WG;
+static constexpr int FZ_POS_PER_TILE = 4 * (1 + 7 * 8);    // ring positions of one tile: 4 stages per k-block, 1 + 7 x 8 k-blocks
+static_assert(FZ_SMEM <= 232448, "dynamic shared memory limit of sm_90");
 
 struct SdfFusedParams {
-  CUtensorMap tmW[8][2];     // layer l, plane p: [512 n-rows] x [Kp] bf16, box {64 k, 128 n}, 128B swizzle
+  CUtensorMap tmW[8][2];     // layer l, plane p: [512 n-rows] x [Kp] bf16, box {64 k, 64 n}, 128B swizzle
   const float* bias[8];
   const float* head_w;       // lin8 row 0 (512)
   const float* head_b;       // its bias
   const float* pts;          // [M, 3]
   float* sdf;                // [M]
-  int M, n_tiles;            // n_tiles counts 128-row pair tiles
+  int M, n_tiles;            // n_tiles counts 64-row tiles
 };
-
-// (Barrier waits / remote arrivals keep the default CTA-scope semantics of the kernels above: the activations live in shared
-//  memory and are read by the tensor core through the async proxy - fence.proxy.async on the writer side - so no L1 is involved;
-//  a cluster-scope acquire compiled to CCTL.IVALL on every a_ready wait and threw the biases out of L1: ncu, first version.)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 512;" ::: "memory"); }   // the 16 epilogue warps of this CTA
 
 // feature f (0..38) of the 6-frequency positional encoding of x[3]: [x, sin(2^k x), cos(2^k x)]_k, as csrc/embed.cu lays it out
 __device__ __forceinline__ float pe6_feature(const float (&x)[3], int f) {
@@ -1118,159 +645,51 @@ __device__ __forceinline__ float pe6_feature(const float (&x)[3], int f) {
   return wi < 3 ? sn : cs;
 }
 
-// MMA unit u of layer l -> (column half h, input k-block kb).  Layer 0 has one k-block: (h0, kb0), (h1, kb0).  Layers 1-7:
-//   units 0-7 : k-blocks 0, 2, 1, 3 for both halves (h0 then h1 per k-block)     - the order in which the previous layer's
-//   units 8-11: half 0 on k-blocks 4, 6, 5, 7 -> commit half 0                      epilogue finishes them (each epilogue warp
-//   units 12-15: half 1 on k-blocks 4, 6, 5, 7 -> commit half 1                     writes an even k-block first, then its odd one)
-__host__ __device__ constexpr int fz_unit_packed(int l, int u) {           // h | kb << 4
-  if (l == 0) return u;
-  const int seq = (0x3120 >> (4 * ((u < 8 ? (u >> 1) : u) & 3))) & 0xF;      // 0, 2, 1, 3
-  return u < 8 ? ((u & 1) | (seq << 4)) : (((u - 8) >> 2) | ((4 + seq) << 4));
-}
-__device__ __forceinline__ void fz_unit(int l, int u, int& h, int& kb) {
-  const int pk = fz_unit_packed(l, u);
-  h = pk & 0xF;
-  kb = pk >> 4;
-}
-// the schedule the in-place activation update relies on, checked at compile time: every (half, k-block) pair exactly once per
-// layer; both halves have consumed k-blocks 0-3 before half 0 commits (after unit 11); half 1's last unit is unit 15
-constexpr bool fz_schedule_ok() {
-  int seen[2][8] = {{0, 0, 0, 0, 0, 0, 0, 0}, {0, 0, 0, 0, 0, 0, 0, 0}};
-  for (int u = 0; u < 16; ++u) {
-    const int pk = fz_unit_packed(1, u), h = pk & 0xF, kb = pk >> 4;
-    if (h > 1 || kb > 7 || seen[h][kb]) return false;
-    seen[h][kb] = 1;
-    if (u < 8 && kb > 3) return false;                    // units 0-7 read k-blocks 0-3 only ...
-    if (u >= 8 && kb < 4) return false;                   // ... and nothing reads them afterwards
-    if (u >= 8 && h != (u - 8) / 4) return false;         // units 8-11 finish half 0, units 12-15 half 1
-  }
-  return fz_unit_packed(0, 0) == 0 && fz_unit_packed(0, 1) == 1;
-}
-static_assert(fz_schedule_ok(), "fused SDF chain: MMA unit schedule");
-__device__ __forceinline__ bool fz_first_kb(int l, int u) { return l == 0 || u < 2; }   // first k-block of an accumulator (no accumulate)
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(640, 1) sdf_fused_kernel(const __grid_constant__ SdfFusedParams p) {
+__global__ void __launch_bounds__(FZ_THREADS, 1) sdf_fused_kernel(const __grid_constant__ SdfFusedParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FZ_BAR);
-  const uint32_t w_full = smem_u32(bars), w_empty = smem_u32(bars + 3), acc_full = smem_u32(bars + 6), a_ready = smem_u32(bars + 8);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 16);     // a_ready[8]: one barrier per input k-block
+  const uint32_t w_full = smem_u32(bars);        // w_full[g * FZ_NST + s]: stage s of warpgroup g's ring
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
   const uint32_t smem0 = smem_u32(smem);
+  const int g = warp >> 2, wi = warp & 3, et = threadIdx.x;
+  const bool loader = wi == 0 && lane == 0;      // issues this warpgroup's weight loads
 
-  if (warp == 0 && lane == 0) {
+  if (et == 0) {
     for (int l = 0; l < 8; ++l) { tma_prefetch_desc(&p.tmW[l][0]); tma_prefetch_desc(&p.tmW[l][1]); }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < FZ_NST; ++i) { mbar_init(w_full + 8 * i, 1); mbar_init(w_empty + 8 * i, 1); }
-    for (int i = 0; i < 2; ++i) mbar_init(acc_full + 8 * i, 1);
-    for (int i = 0; i < 8; ++i) mbar_init(a_ready + 8 * i, 16);   // the 8 epilogue warps per CTA that write k-block i, both CTAs
+    for (int i = 0; i < FZ_WG * FZ_NST; ++i) mbar_init(w_full + 8 * i, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
   pdl_launch_dependents();
 
-  const int unit = blockIdx.x >> 1, n_units = gridDim.x >> 1;
+  // ring position pos of this warpgroup (tile, layer, k-block kb, u = 2 h + (hi-plane weights)) -> TMA load into stage pos % FZ_NST
+  auto load = [&](int pos) {
+    const int tile = blockIdx.x + (pos / FZ_POS_PER_TILE) * gridDim.x;
+    if (tile >= p.n_tiles) return;
+    const int q = pos % FZ_POS_PER_TILE;
+    const int l = q < 4 ? 0 : 1 + (q - 4) / 32, r = q < 4 ? q : (q - 4) % 32;
+    const int kb = r >> 2, u = r & 3;
+    const uint32_t st = g * FZ_NST + pos % FZ_NST;
+    mbar_arrive_expect_tx(w_full + 8 * st, FZ_WSTAGE);
+    tma_load_2d(smem0 + FZ_A + st * FZ_WSTAGE, &p.tmW[l][(u & 1) ? 0 : 1], w_full + 8 * st, kb * BK, 128 * g + 64 * (u >> 1));
+  };
+  if (loader)
+    for (int i = 0; i < FZ_NST; ++i) load(i);
 
-  if (warp == 0) {
-    // ===================== weight producer (both CTAs: each streams its 128 of the 256 weight rows of an MMA) =====================
-    const bool issuer = elect_one();
-    int s = 0;
-    uint32_t ph = 0;
-    for (int tile = unit; tile < p.n_tiles; tile += n_units) {
-      for (int l = 0; l < 8; ++l) {
-        const int nu = l == 0 ? 2 : 16;
-        for (int u = 0; u < nu; ++u) {
-          int h, kb;
-          fz_unit(l, u, h, kb);
-          mbar_wait(w_empty + 8 * s, ph ^ 1);
-          if (issuer) {
-            if (leader) mbar_arrive_expect_tx(w_full + 8 * s, 2 * FZ_WSTAGE);
-            const uint32_t bfl = (w_full + 8 * s) & PEER_MASK;
-            const uint32_t dst = smem0 + FZ_A + s * FZ_WSTAGE;
-            const int n0 = h * 256 + (int)rank * 128;
-            tma_load_2d_2sm(dst, &p.tmW[l][0], bfl, kb * BK, n0);
-            tma_load_2d_2sm(dst + FZ_WPL, &p.tmW[l][1], bfl, kb * BK, n0);
-          }
-          __syncwarp();
-          if (++s == FZ_NST) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA) =====================
-    if (leader) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      const uint64_t desc_hi = make_sdesc(0, 16, 1024);
-      const bool issuer = elect_one();
-      int s = 0;
-      uint32_t ph = 0, pa = 0;                   // pa: phase bit of a_ready[kb] at bit kb
-      for (int tile = unit; tile < p.n_tiles; tile += n_units) {
-        for (int l = 0; l < 8; ++l) {
-          const uint32_t acc = tmem_base + (uint32_t)(l & 1) * 256u;
-          uint32_t seen = 0;                     // k-blocks of this layer's input already waited for
-          const int nu = l == 0 ? 2 : 16;
-          for (int u = 0; u < nu; ++u) {
-            int h, kb;
-            fz_unit(l, u, h, kb);
-            if (!((seen >> kb) & 1u)) {          // input k-block kb (layer 0: the encoded points) is in shared memory
-              mbar_wait(a_ready + 8 * kb, (pa >> kb) & 1u);
-              pa ^= 1u << kb;
-              seen |= 1u << kb;
-              tc_fence_after();
-            }
-            mbar_wait(w_full + 8 * s, ph);
-            tc_fence_after();
-            if (issuer) {
-              const uint32_t sa = smem0 + kb * (FZ_ROWS * BK * 2);
-              const uint32_t sb = smem0 + FZ_A + s * FZ_WSTAGE;
-              uint32_t accum = !fz_first_kb(l, u);
-#pragma unroll
-              for (int pr = 0; pr < 3; ++pr) {   // (hi, lo), (lo, hi), (hi, hi): the product order of the per-layer kernels
-                const uint32_t pa = pr == 1 ? 1u : 0u, pb = pr == 0 ? 1u : 0u;
-                const uint64_t da = desc_hi | (uint64_t)(((sa + pa * FZ_APLANE) & 0x3FFFFu) >> 4);
-                const uint64_t db = desc_hi | (uint64_t)(((sb + pb * FZ_WPL) & 0x3FFFFu) >> 4);
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                  umma_bf16_2sm(acc + (uint32_t)h * 128u, da + ((k * 32) >> 4), db + ((k * 32) >> 4), idesc, accum);
-                  accum = 1;
-                }
-              }
-              umma_commit_2sm(w_empty + 8 * s);
-              if (l == 0 || u == 11 || u == 15) umma_commit_2sm(acc_full + 8 * h);
-            }
-            __syncwarp();
-            if (++s == FZ_NST) { s = 0; ph ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (both CTAs, own 64 rows) =====================
-    const int ew = warp - 4, q = warp & 3, chalf = ew >> 2, et = threadIdx.x - 128;
-    const int row = 32 * (q & 1) + lane;                       // TMEM lanes 0-63: columns 0-127 of the MMA, lanes 64-127: columns 128-255
-    const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-    const int colq = 128 * (q >> 1);
-    const int rsw = row & 7;
-    float* part = reinterpret_cast<float*>(smem + FZ_PART);
-    uint32_t pacc = 0;
-    for (int tile = unit; tile < p.n_tiles; tile += n_units) {
-      const int m0 = tile * 128 + (int)rank * FZ_ROWS;
+  {
+    // ===================== warpgroup g: output columns 128 g .. 128 g + 127 of every layer =====================
+    const int r0 = 16 * wi + (lane >> 2), c0 = 2 * (lane & 3);   // fragment rows r0, r0 + 8; columns 8 j + c0 + {0, 1}
+    const uint64_t desc_hi = make_gdesc(0, 16, 1024);
+    float* part = reinterpret_cast<float*>(smem);                 // head partials [64 rows][4], over k-block 0 once layer 7 has read it
+    int pos = 0;                                                  // ring position consumed next
+    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+      const int m0 = tile * FZ_ROWS;
       // ---- layer-0 input: positional encoding of this CTA's 64 points, written as the k-block-0 tiles of both planes ----
       *reinterpret_cast<uint4*>(smem + et * 16) = make_uint4(0, 0, 0, 0);
       *reinterpret_cast<uint4*>(smem + FZ_APLANE + et * 16) = make_uint4(0, 0, 0, 0);
-      epi_bar_sync();
+      named_bar_sync(1, 128 * FZ_WG);
       if (et < 3 * FZ_ROWS) {
         const int r = et / 3, c = et % 3, m = m0 + r;
         const float x = m < p.M ? __ldg(p.pts + (long long)m * 3 + c) : 0.0f;
@@ -1290,108 +709,118 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(640, 1) sdf_fused_ke
         }
       }
       fence_proxy_async_smem();
-      tc_fence_before();                       // the head epilogue of the previous tile has drained its accumulators
-      epi_bar_sync();                          // every warp's part of the tile is written (and fenced) ...
-      if ((q >> 1) == 0 && lane == 0) mbar_arrive_leader(a_ready);   // ... the 8 warps that own k-block 0 signal it
-      const int mrow = m0 + row;
+      named_bar_sync(1, 128 * FZ_WG);
+      float hsum[2] = {0.0f, 0.0f};
       for (int l = 0; l < 8; ++l) {
-        const uint32_t acc = tmem_base + (uint32_t)(l & 1) * 256u;
-        const float* bias = p.bias[l];
-        for (int h = 0; h < 2; ++h) {
-          mbar_wait(acc_full + 8 * h, pacc);
-          tc_fence_after();
-          float hsum = 0.0f;
-          // both of this warp's 16-column chunks leave the TMEM together (one wait), the first bias vector rides along
-          float va[16], vb[16];
-          tmem_ld16_issue(acc + (uint32_t)(h * 128 + 16 * chalf) + lane_sel, va);
-          tmem_ld16_issue(acc + (uint32_t)(h * 128 + 16 * (chalf + 4)) + lane_sel, vb);
-          auto chunk = [&](float (&v)[16], const int cc) {
-            const int c = chalf + 4 * cc;
-            const int n = 256 * h + colq + 16 * c;             // first of this thread's 16 output columns
-            float b[16];
+        const int nkb = l == 0 ? 1 : 8;
+        float acc0[32], acc1[32];                 // columns 128 g + [0, 64) and 128 g + [64, 128)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float4 t = __ldg(reinterpret_cast<const float4*>(bias + n) + i);
-              b[4 * i] = t.x; b[4 * i + 1] = t.y; b[4 * i + 2] = t.z; b[4 * i + 3] = t.w;
+        for (int i = 0; i < 32; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+        // one ring stage: u = 2 h + (hi-plane weights); lo-plane weights carry product (hi, lo), hi-plane ones (lo, hi), (hi, hi)
+        auto stage = [&](float (&ah)[32], const uint32_t sa, const int u) {
+          const uint32_t st = g * FZ_NST + pos % FZ_NST;
+          mbar_wait(w_full + 8 * st, (pos / FZ_NST) & 1);
+          const uint64_t db = desc_hi | (uint64_t)(((smem0 + FZ_A + st * FZ_WSTAGE) & 0x3FFFFu) >> 4);
+          wgmma_fence();
+          if ((u & 1) == 0) {
+            const uint64_t da = desc_hi | (uint64_t)((sa & 0x3FFFFu) >> 4);
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) wgmma_bf16<64, 0, 0>(ah, da + 2 * k, db + 2 * k, 1u);
+          } else {
+#pragma unroll
+            for (int pa = 1; pa >= 0; --pa) {
+              const uint64_t da = desc_hi | (uint64_t)(((sa + pa * FZ_APLANE) & 0x3FFFFu) >> 4);
+#pragma unroll
+              for (int k = 0; k < BK / 16; ++k) wgmma_bf16<64, 0, 0>(ah, da + 2 * k, db + 2 * k, 1u);
             }
-            if (cc == 0) tmem_ld_wait();
-            if (l == 7) {                                      // sdf head: fixed-order partial dot product with lin8's row 0
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float4 hw = __ldg(reinterpret_cast<const float4*>(p.head_w + n) + i);
-                hsum = fmaf(softplus100(v[4 * i] + b[4 * i]), hw.x, hsum);
-                hsum = fmaf(softplus100(v[4 * i + 1] + b[4 * i + 1]), hw.y, hsum);
-                hsum = fmaf(softplus100(v[4 * i + 2] + b[4 * i + 2]), hw.z, hsum);
-                hsum = fmaf(softplus100(v[4 * i + 3] + b[4 * i + 3]), hw.w, hsum);
-              }
-              return;
-            }
-            float (&w)[16] = v;
-            if (l == 3) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) w[i] = softplus100(v[i] + b[i]) * 0.70710678118654752440f;
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) w[i] = softplus100(v[i] + b[i]) * 1.0f;
-            }
-            uint32_t hi[8], lo[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const __nv_bfloat162 hh = __floats2bfloat162_rn(w[2 * i], w[2 * i + 1]);
-              const float2 hf = __bfloat1622float2(hh);
-              const __nv_bfloat162 ll = __floats2bfloat162_rn(w[2 * i] - hf.x, w[2 * i + 1] - hf.y);
-              hi[i] = *reinterpret_cast<const uint32_t*>(&hh);
-              lo[i] = *reinterpret_cast<const uint32_t*>(&ll);
-            }
-            uint8_t* dst = smem + (n >> 6) * (FZ_ROWS * BK * 2) + row * 128;
-            const int ch0 = (n & 63) >> 3;
-            const int o0 = ((ch0 ^ rsw) << 4), o1 = (((ch0 + 1) ^ rsw) << 4);
-            *reinterpret_cast<uint4*>(dst + o0) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            *reinterpret_cast<uint4*>(dst + o1) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-            *reinterpret_cast<uint4*>(dst + FZ_APLANE + o0) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-            *reinterpret_cast<uint4*>(dst + FZ_APLANE + o1) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-            if (l == 3 && n + 15 >= 473) {                     // skip connection: columns 473-511 of layer 4's input = PE(x) / sqrt(2)
-              float x[3];
-#pragma unroll
-              for (int i = 0; i < 3; ++i) x[i] = mrow < p.M ? __ldg(p.pts + (long long)mrow * 3 + i) : 0.0f;
-#pragma unroll 1
-              for (int i = n < 473 ? 473 - n : 0; i < 16; ++i) {       // overwrites what the same thread stored above
-                const float pv = pe6_feature(x, n + i - 473) * 0.70710678118654752440f;
-                const bf16 ph = __float2bfloat16_rn(pv), pl = __float2bfloat16_rn(pv - __bfloat162float(ph));
-                const int off = ((((ch0 + (i >> 3)) ^ rsw)) << 4) + (i & 7) * 2;
-                *reinterpret_cast<bf16*>(dst + off) = ph;
-                *reinterpret_cast<bf16*>(dst + FZ_APLANE + off) = pl;
-              }
-            }
-            // this warp's 32 rows x 16 columns of k-block n / 64 are written: 8 warps per CTA complete a k-block
-            fence_proxy_async_smem();          // generic-proxy stores -> visible to the tensor core's reads
-            if (cc == 1) tc_fence_before();    // (after the last TMEM read of this accumulator half)
-            __syncwarp();
-            if (lane == 0) mbar_arrive_leader(a_ready + 8 * (n >> 6));
-          };
-          chunk(va, 0);
-          chunk(vb, 1);
-          if (l == 7) part[row * 16 + h * 8 + (q >> 1) * 4 + chalf] = hsum;
+          }
+          wgmma_commit();
+          acc_fence(acc0);
+          acc_fence(acc1);
+          if (pos > 0) {                          // the previous stage's MMAs have completed: refill it, two positions ahead
+            wgmma_wait<1>();
+            acc_fence(acc0);
+            acc_fence(acc1);
+            if (loader) load(pos + FZ_NST - 1);
+          }
+          ++pos;
+        };
+        for (int kb = 0; kb < nkb; ++kb) {
+          const uint32_t sa = smem0 + kb * (FZ_ROWS * BK * 2);
+          stage(acc0, sa, 0);
+          stage(acc0, sa, 1);
+          stage(acc1, sa, 2);
+          stage(acc1, sa, 3);
         }
-        pacc ^= 1;
+        wgmma_wait<0>();
+        acc_fence(acc0);
+        acc_fence(acc1);
+        named_bar_sync(1, 128 * FZ_WG);           // every warpgroup has read this layer's input: it may be overwritten
+        const float* bias = p.bias[l];
+        if (l == 7) {                             // sdf head: fixed-order partial dot product with lin8's row 0
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int n = 128 * g + 8 * j + c0;
+            const float2 b = __ldg(reinterpret_cast<const float2*>(bias + n));
+            const float2 hw = __ldg(reinterpret_cast<const float2*>(p.head_w + n));
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              const float* a = j < 8 ? acc0 + 4 * j : acc1 + 4 * (j - 8);
+              hsum[rr] = fmaf(softplus100(a[2 * rr] + b.x), hw.x, hsum[rr]);
+              hsum[rr] = fmaf(softplus100(a[2 * rr + 1] + b.y), hw.y, hsum[rr]);
+            }
+          }
+          break;
+        }
+        const float scale = l == 3 ? 0.70710678118654752440f : 1.0f;
+        float x[2][3];                            // skip connection: columns 473-511 of layer 4's input = PE(x) / sqrt(2)
+        if (l == 3 && g == 3) {
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int m = m0 + r0 + 8 * rr;
+#pragma unroll
+            for (int i = 0; i < 3; ++i) x[rr][i] = m < p.M ? __ldg(p.pts + (long long)m * 3 + i) : 0.0f;
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int n = 128 * g + 8 * j + c0;
+          const float2 b = __ldg(reinterpret_cast<const float2*>(bias + n));
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int row = r0 + 8 * rr;
+            const float* a = j < 8 ? acc0 + 4 * j : acc1 + 4 * (j - 8);
+            float w0 = softplus100(a[2 * rr] + b.x) * scale, w1 = softplus100(a[2 * rr + 1] + b.y) * scale;
+            if (l == 3 && n + 1 >= 473) {
+              if (n >= 473) w0 = pe6_feature(x[rr], n - 473) * 0.70710678118654752440f;
+              w1 = pe6_feature(x[rr], n + 1 - 473) * 0.70710678118654752440f;
+            }
+            const __nv_bfloat162 hh = __floats2bfloat162_rn(w0, w1);
+            const float2 hf = __bfloat1622float2(hh);
+            const __nv_bfloat162 ll = __floats2bfloat162_rn(w0 - hf.x, w1 - hf.y);
+            const int off = (n >> 6) * (FZ_ROWS * BK * 2) + row * 128 + ((((n & 63) >> 3) ^ (row & 7)) << 4) + (n & 7) * 2;
+            *reinterpret_cast<__nv_bfloat162*>(smem + off) = hh;
+            *reinterpret_cast<__nv_bfloat162*>(smem + FZ_APLANE + off) = ll;
+          }
+        }
+        fence_proxy_async_smem();                 // generic-proxy stores -> visible to the next layer's wgmma
+        named_bar_sync(1, 128 * FZ_WG);
       }
-      // ---- sdf = sum of the 16 column partials in a fixed order + bias ----
-      epi_bar_sync();
+      // ---- sdf = the four warpgroups' partials in a fixed order + bias ----
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        hsum[rr] += __shfl_xor_sync(0xFFFFFFFFu, hsum[rr], 1);
+        hsum[rr] += __shfl_xor_sync(0xFFFFFFFFu, hsum[rr], 2);
+        if ((lane & 3) == 0) part[(r0 + 8 * rr) * 4 + g] = hsum[rr];
+      }
+      named_bar_sync(1, 128 * FZ_WG);
       if (et < FZ_ROWS) {
-        const float4* pr4 = reinterpret_cast<const float4*>(part + et * 16);
-        const float4 a = pr4[0], b4 = pr4[1], c4 = pr4[2], d4 = pr4[3];
-        const float sum = (((a.x + a.y) + (a.z + a.w)) + ((b4.x + b4.y) + (b4.z + b4.w))) + (((c4.x + c4.y) + (c4.z + c4.w)) + ((d4.x + d4.y) + (d4.z + d4.w)));
+        const float4 a = *reinterpret_cast<const float4*>(part + et * 4);
         const int m = m0 + et;
-        if (m < p.M) p.sdf[m] = sum + __ldg(p.head_b);
+        if (m < p.M) p.sdf[m] = ((a.x + a.y) + (a.z + a.w)) + __ldg(p.head_b);
       }
+      named_bar_sync(1, 128 * FZ_WG);             // the partials are read before the next tile's encoding overwrites them
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
   }
 }
 
@@ -1402,11 +831,11 @@ int sdf_fused_forward(const SdfFusedDesc& d, cudaStream_t stream) {
   for (int l = 0; l < 8; ++l) {
     const int K = l == 0 ? 64 : 512;
     NRW_CHECK(d.W[l].p && d.W[l].ld == K && d.bias[l], NRW_ERR_ARG, "sdf_fused_forward: layer %d needs packed [512 x %d] weights (ld=%d)", l, K, d.W[l].ld);
-    for (int pl = 0; pl < 2; ++pl) NRW_TRY(make_map(&p.tmW[l][pl], d.W[l].plane(pl), K, 512, d.W[l].ld, BK, 128));
+    for (int pl = 0; pl < 2; ++pl) NRW_TRY(make_map(&p.tmW[l][pl], d.W[l].plane(pl), K, 512, d.W[l].ld, BK, 64));
     p.bias[l] = d.bias[l];
   }
   p.head_w = d.head_w; p.head_b = d.head_b; p.pts = d.pts; p.sdf = d.sdf; p.M = d.M;
-  p.n_tiles = cdiv(d.M, 2 * FZ_ROWS);
+  p.n_tiles = cdiv(d.M, FZ_ROWS);
   static int n_sm_dev[MAX_DEV] = {0};
   static bool attr_set[MAX_DEV] = {false};
   const int dev = current_device();
@@ -1415,13 +844,13 @@ int sdf_fused_forward(const SdfFusedDesc& d, cudaStream_t stream) {
     NRW_CUDA_OK(cudaFuncSetAttribute(sdf_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FZ_SMEM));
     attr_set[dev] = true;
   }
-  int pairs = n_sm_dev[dev] / 2;
-  if (p.n_tiles < pairs) pairs = p.n_tiles;
+  int grid = n_sm_dev[dev];
+  if (p.n_tiles < grid) grid = p.n_tiles;
   static const int pdl = getenv("NRW_PDL") ? atoi(getenv("NRW_PDL")) : 1;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2 * pairs, 1, 1);
-  cfg.blockDim = dim3(640, 1, 1);
+  cfg.gridDim = dim3(grid, 1, 1);
+  cfg.blockDim = dim3(FZ_THREADS, 1, 1);
   cfg.dynamicSmemBytes = FZ_SMEM;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];

@@ -55,7 +55,7 @@ int grad_sumsq(const float* g, long long n, double* acc, cudaStream_t s) {
   if (n <= 0) return NRW_OK;
   const int T = 256;
   long long blocks = (n + T - 1) / T;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;   // 8 blocks per SM of an H100 SXM
   sumsq_kernel<<<(int)blocks, T, 0, s>>>(g, n, acc);
   NRW_LAUNCH_OK();
   return NRW_OK;
@@ -70,7 +70,7 @@ int adam_clip_step(float* p, const float* g, float* m, float* v, long long n, co
   const double bc2 = 1.0 - pow(b2, (double)step);
   const int T = 256;
   long long blocks = (n + T - 1) / T;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   adam_clip_kernel<<<(int)blocks, T, 0, s>>>(p, g, m, v, n, sumsq, (float)max_norm, (float)(lr / bc1), (float)(1.0 - b1), (float)b2,
                                              (float)(1.0 - b2), (float)eps, (float)sqrt(bc2));
   NRW_LAUNCH_OK();

@@ -47,8 +47,7 @@ class Engine:
         if self.bwd_planes:
             check(self.L.nrw_ctx_set_backward_planes(self.ctx, self.bwd_planes), "nrw_ctx_set_backward_planes")
         # backward sweeps rebuild softplus'(a) / softplus''(a) from the stored output planes: with plain-bf16 backward GEMMs
-        # ('mixed') the hi plane alone is enough (gradient cosine vs the fp32 reference 0.9999998 either way,
-        # profiles/r2_precision_study.json); the strict modes read every plane
+        # ('mixed') the hi plane alone is enough (tests/test_gpu_precision_policy.py); the strict modes read every plane
         gate = int(os.environ.get("NRW_BWD_GATE_PLANES", 1 if self.bwd_planes == 1 else 0))
         if gate:
             check(self.L.nrw_ctx_set_backward_gate_planes(self.ctx, min(gate, self.n_planes)), "nrw_ctx_set_backward_gate_planes")
@@ -103,7 +102,7 @@ class Engine:
     def ensure(self, device, max_rays, max_T, with_backward, S=None, chunk_hint=0):
         """(Re)bind the workspace.  With backward enabled, as many chunk slots as the memory budget
         (NRW_SLOT_BUDGET_GB, default 60 % of free HBM) allows keep their forward activations resident so
-        the backward pass does not recompute the forward (the 180 GB of a B200 hold a full 8192x128 batch).
+        the backward pass does not recompute the forward (when the HBM holds all chunks of the batch).
 
         Bounds only ever grow.  `max_rays x max_T` sizes the PER-RAY scratch of render / sample; point queries
         (sdf, neuconw_forward, nerf_forward) need chunk buffers only and pass `chunk_hint` (rows they would like one

@@ -168,5 +168,82 @@ def main():
         print(f"wrote {path}: loss={float(loss):.6f} {os.path.getsize(path) / 1024:.1f} KiB")
 
 
+
+
+# ---- reference results the CPU tests of the ports compare against (tests/test_oracle_vs_reference.py, tests/test_dataio_oracle.py)
+REF_CHECKS = os.path.join(GOLDEN_DIR, "reference_checks.npz")
+LIVE_CFG = dict(n_samples=12, n_importance=12, up_sample_steps=3, n_outside=6, s_val_base=2, cos_anneal_ratio=0.25)
+LIVE_RAYS, LIVE_SEED = 24, 5
+SPLIT_CASES = [(64, 8), (64, 3), (5, 4), (7, 1)]
+RANGE_CASES = [(10, 4), (12, 4), (1, 3)]
+FULL_GRAD_NUMEL = 2048          # gradients up to this size are stored whole, larger ones as a seeded sample of 1024 elements
+
+
+def grad_sample_index(name, numel, n=1024):
+    gen = torch.Generator().manual_seed(7 + sum(map(ord, name)) % 100003)
+    return torch.randperm(numel, generator=gen)[:n]
+
+
+def getitem_inputs():
+    """seeded ray table + index sample of the getitem / filter check"""
+    g = torch.Generator().manual_seed(0)
+    n = 500
+    all_rays = torch.randn(n, 12, generator=g)
+    all_rays[:, 8] = torch.randint(0, 1500, (n,), generator=g).float()
+    all_rays[:, 9] = torch.tensor([0.0, 2.0, 12.0, 20.0, 116.0, 127.0, 6.0])[torch.randint(0, 7, (n,), generator=g)]
+    all_rgbs = torch.rand(n, 3, generator=g)
+    idx = torch.randperm(n, generator=g)[:97]
+    return all_rays, all_rgbs, idx
+
+
+def reference_checks():
+    import json
+    import types
+
+    ref_import.load()
+    from datasets.data import DataModule  # type: ignore
+    from datasets.mask_utils import get_label_id_mapping  # type: ignore
+    from datasets.phototourism import PhototourismDataset  # type: ignore
+    from utils.visualization import get_local_split  # type: ignore
+
+    from oracle import dataio_port as dp
+
+    arrays = {}
+    P = synth.make_params(seed=0)
+    cfg = synth.PathConfig(**LIVE_CFG, **synth.BRANDENBURG)
+    batch = synth.make_rays(LIVE_RAYS, cfg, seed=LIVE_SEED)
+    res, loss, grads, m = reference_train_step(cfg, P, batch, perturb_overwrite=0)
+    arrays.update({f"live.out.{k}": v.detach().numpy() for k, v in res.items()})
+    arrays["live.loss"] = loss.numpy()
+    for k, g in grads.items():
+        if g.numel() <= FULL_GRAD_NUMEL:
+            arrays["live.g." + k] = g.numpy()
+        else:                   # a seeded sample of the elements + the tensor's max magnitude (the tolerance scale)
+            arrays["live.gs." + k] = g.reshape(-1)[grad_sample_index(k, g.numel())].numpy()
+            arrays["live.gmax." + k] = g.abs().max().numpy()
+    names = {}
+    for pre, mod in (("neuconw.", m["neuconw"]), ("nerf.", m["nerf"]), ("embedding_a.", m["emb"])):
+        for k, v in mod.state_dict().items():
+            names[pre + k] = list(v.shape)
+    arrays["state_dict_shapes"] = np.array(json.dumps(names, sort_keys=True))
+    for n_items, world in SPLIT_CASES:
+        items = [f"split_{i}" for i in range(n_items)]
+        arrays[f"split.{n_items}.{world}"] = np.array(json.dumps([list(DataModule._get_local_split(None, items, world, r)) for r in range(world)]))
+    all_rays, all_rgbs, idx = getitem_inputs()
+    fake = types.SimpleNamespace(split="train", all_rays=all_rays, all_rgbs=all_rgbs, with_semantics=True)
+    items = [PhototourismDataset.__getitem__(fake, int(i)) for i in idx]
+    for k in items[0]:
+        arrays["getitem." + k] = torch.stack([it[k] for it in items]).numpy()
+    mapping = get_label_id_mapping()
+    arrays["label_ids"] = np.array(json.dumps({k: mapping[k] for k in dp.LABEL_IDS}, sort_keys=True))
+    for n, world in RANGE_CASES:
+        data = torch.arange(n * 3, dtype=torch.float32).reshape(n, 3) + 1
+        for rank in range(world):
+            arrays[f"range.{n}.{world}.{rank}"] = get_local_split(data, world, rank).numpy()
+    np.savez_compressed(REF_CHECKS, **arrays)
+    print(f"wrote {REF_CHECKS}: {os.path.getsize(REF_CHECKS) / 1024:.1f} KiB")
+
+
 if __name__ == "__main__":
     main()
+    reference_checks()

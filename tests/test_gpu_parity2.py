@@ -58,7 +58,7 @@ def install_injected_hits(renderer, hits):
 # ------------------------------------------------------------------------------------------------------------
 def test_train_step_c2_sample_counts(P):
     """BASELINE C2 counts (64 coarse + 64 importance in 4 rounds + 4 outside -> S=128, T=132), brandenburg frame,
-    perturbed strata with injected draws, R=64, bf16x3 tcgen05 path vs the oracle port: 1e-4 on every dict key."""
+    perturbed strata with injected draws, R=64, bf16x3 tensor-core path vs the oracle port: 1e-4 on every dict key."""
     cfg = synth.PathConfig(perturb=1.0, **synth.BRANDENBURG)
     assert (cfg.n_samples, cfg.n_importance, cfg.up_sample_steps, cfg.n_outside) == (64, 64, 4, 4)
     R = 64
@@ -135,7 +135,7 @@ def test_cuda_vs_reference_golden_perturb_and_fine(P, name):
 
 # ------------------------------------------------------------------------------------------------------------
 def test_sampler_index_mismatch_rate_reported(P):
-    """Whole CUDA sampler (tcgen05 SDF queries inside) at C2 counts vs the reference ops (oracle port, fp32 SDF):
+    """Whole CUDA sampler (tensor-core SDF queries inside) at C2 counts vs the reference ops (oracle port, fp32 SDF):
     searchsorted indices of every up-sampling round.  Given IDENTICAL sdf inputs the CUDA round is bit-exact against
     the written-down restatement and that restatement has 0 mismatches against torch on the seeded cases
     (tests/test_sampler_oracle.py); what is measured here is the effect of the SDF's 1e-6 differences."""

@@ -1,5 +1,5 @@
 """GPU: the fused forward-only SDF chain (gemm_tc.cu::sdf_fused_kernel, models/neuconw.py:263-282 in one kernel) against
-(a) the torch-CPU oracle, (b) the per-layer tcgen05 chain it replaces (NRW_SDF_FUSED=0, separate process: the switch is read
+(a) the torch-CPU oracle, (b) the per-layer tensor-core chain it replaces (NRW_SDF_FUSED=0, separate process: the switch is read
 once), on ragged sizes around the 64-row CTA tile and the 128-row pair tile, and (c) itself (run-to-run bit-identical)."""
 import os
 import subprocess

@@ -1,4 +1,4 @@
-"""Micro-benchmarks of the tcgen05 GEMM through the C ABI test hook (CUDA-event timed)."""
+"""Micro-benchmarks of the tensor-core GEMM through the C ABI test hook (CUDA-event timed)."""
 import ctypes as C, os, sys, argparse
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "neuralrecon-w_b200"))
