@@ -326,12 +326,13 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const floa
   }
 }
 
-// Column-sum accumulator of one CTA (<= 256 columns of the current n-tile).  All `n_threads` epilogue threads call
-// this together (named barrier `bar_id`): adds the tile's partial sums to global memory and clears the accumulator.
+// Column-sum accumulator of one consumer warpgroup (the n_cols columns of its current n-tile; the chunk epilogues never
+// touch an entry beyond n_cols, so those stay zero).  All `n_threads` threads of the warpgroup call this together (named
+// barrier `bar_id`): adds the tile's partial sums to global memory and clears the accumulator.
 __device__ __forceinline__ void colsum_flush(float* cs, float* __restrict__ colsum, int n0, int n_cols, int tid, int n_threads,
                                              int bar_id) {
   asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(n_threads) : "memory");
-  for (int i = tid; i < 256; i += n_threads) {
+  for (int i = tid; i < n_cols; i += n_threads) {
     const float s = cs[i];
     if (i < n_cols && s != 0.0f) atomicAdd(colsum + n0 + i, s);
     cs[i] = 0.0f;

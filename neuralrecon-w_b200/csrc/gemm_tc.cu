@@ -6,12 +6,17 @@
 //   n_planes=2 issues hi*hi + hi*lo + lo*hi (~16 mantissa bits), n_planes=3 all six
 //   products whose weight is >= 2^-16 (~fp32).  All products accumulate into the same fp32
 //   register accumulator, so precision is a loop bound, not a different kernel.
-// * persistent CTAs (one per SM), warp-specialised: warps 0-7 = two consumer warpgroups (each
-//   wgmma.m64nBNk16 on its 64 rows of the 128-row tile, then the epilogue of those rows), warp 8 =
-//   TMA producer.  smem ring of TMA stages (128B swizzle) so the loads of the next k-blocks (and of
-//   the next tile) overlap the MMAs and the epilogue.
-// * the epilogue stages a warpgroup's accumulators through shared memory into the row layout the
-//   chunk epilogues take (epilogue_tc.cuh / epilogue_fast.cuh: one 32-row x 16-column chunk per warp).
+// * persistent CTAs (one per SM), warp-specialised ping-pong: warps 0-7 = two consumer warpgroups, warps 8-11 =
+//   producer warpgroup (one thread issues the TMA).  A CTA's work items (128 x BN tiles, or tile x K-slice)
+//   alternate between the consumer warpgroups: warpgroup wg takes items blockIdx.x + (2 i + wg) gridDim.x and
+//   runs the whole tile (two wgmma.m64nBNk16 per k16 step, one per 64-row half: 2 x BN/2 fp32 accumulators).
+//   An ordered math barrier hands the tensor cores from one warpgroup's main loop to the other's, so the
+//   epilogue of item i runs while the other warpgroup's MMAs of item i+1 do.  setmaxnreg moves registers from
+//   the producer warpgroup (40) to the consumers (232).
+// * one smem ring of TMA stages (128B swizzle), filled in item order, so the loads of the next k-blocks (and of
+//   the next items) overlap the MMAs and the epilogues.  A stage has a single consuming warpgroup.
+// * the epilogue stages a warpgroup's accumulators (one 64-row half at a time) through shared memory into the row
+//   layout the chunk epilogues take (epilogue_tc.cuh / epilogue_fast.cuh: one 32-row x 16-column chunk per warp).
 // * mn_major=1 consumes both operands "transposed" straight from their natural row-major
 //   [rows=K][cols=M|N] layout (MN-major wgmma descriptors) - used for weight gradients
 //   dW = dY^T X with split-K over the sample dimension and fp32 atomics in the epilogue.
@@ -32,11 +37,14 @@ static constexpr int BM = 128;
 static constexpr int BK = 64;                          // 64 bf16 = 128 B = one swizzle row
 static constexpr int RING_BYTES = 192 * 1024;          // TMA stages
 static constexpr int MAX_STAGES = 8;
-static constexpr int N_CONSUMER_WARPS = 8;             // two warpgroups of 64 rows each
-static constexpr int N_THREADS = 32 * N_CONSUMER_WARPS + 32;
+static constexpr int N_CONSUMER_WARPS = 8;             // two ping-pong warpgroups, each owning whole 128-row tiles
+static constexpr int N_THREADS = 32 * N_CONSUMER_WARPS + 128;   // + the producer warpgroup
+static constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // setmaxnreg split: 128 x 40 + 256 x 232 <= 65536
 static constexpr int EPI_LD = 36;                      // staging row pitch in floats: 32 columns + 4 (16-byte aligned rows)
 static constexpr int EPI_WG_BYTES = 64 * EPI_LD * 4;   // one warpgroup's staging tile [64 rows][32 columns]; doubles as 4 x 2 KB warp tiles
-static constexpr int CS_BYTES = 1024;                  // per-CTA column-sum accumulator (256 columns of one n-tile)
+static constexpr int CS_BYTES = 1024;                  // column-sum accumulators: 128 columns of the current n-tile per warpgroup
+static constexpr int BAR_TURN = 4;                     // named barriers 4 + wg: warpgroup wg's turn at the tensor cores
+static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 32 * N_CONSUMER_WARPS <= 65536, "register file");
 static constexpr int BAR_BYTES = 256;                  // 2 x MAX_STAGES mbarriers
 static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + 2 * EPI_WG_BYTES + CS_BYTES;
 static_assert(SMEM_BYTES <= 232448, "dynamic shared memory limit of sm_90");
@@ -51,8 +59,9 @@ struct TcParams {
   int m_tiles, n_tiles;
   Epi epi;
   // optional cycle attribution (debug): per CTA 16 counters
-  //  [0] producer: waiting for a free stage   [1] consumer warp 0: waiting for TMA data   [4] consumer warp 0: epilogue
-  //  [5] kernel cycles   [6] tiles
+  //  [0] producer: waiting for a free stage   [5] kernel cycles
+  //  first warp of consumer warpgroup wg, o = 8 wg: [1 + o] waiting for TMA data   [3 + o] waiting for its turn at the
+  //  tensor cores   [4 + o] epilogue   [6 + o] tiles
   unsigned long long* prof;
 };
 #define NRW_PROF_T0(cond) const long long _t0 = (cond) ? clock64() : 0
@@ -107,6 +116,13 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 // named barrier over `n` threads (id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// arrive without waiting: the barrier completes once the waiting side's bar.sync threads join
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// per-thread register budget of the executing warpgroup (all its threads execute it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 // generic-proxy shared-memory stores -> visible to the tensor core's (async proxy) reads
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -193,7 +209,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
   static_assert(BN == 64 || BN == 128, "wgmma tile width");
   constexpr int A_TILE = BM * BK * 2;
   constexpr int B_TILE = BN * BK * 2;
-  constexpr int WG_A = 64 * BK * 2;           // one warpgroup's 64 rows of the A tile (K-major: 64 rows; MN-major: one 64-wide slab)
+  constexpr int WG_A = 64 * BK * 2;           // one 64-row half of the A tile (K-major: 64 rows; MN-major: one 64-wide slab)
   extern __shared__ uint8_t smem_raw[];
   // align inside the shared window by OFFSET (an integer round trip of the pointer would turn every staging access
   // into a generic LD/ST instead of LDS/STS)
@@ -216,7 +232,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     }
     for (int i = 0; i < MAX_STAGES; ++i) {
       mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, N_CONSUMER_WARPS);
+      mbar_init(bar_empty + 8 * i, 4);              // the four warps of the stage's consuming warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -230,9 +246,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
   const int n_items = p.m_tiles * p.n_tiles * p.k_slices;
   const int n_prod = (P == 1) ? 1 : (P == 2 ? 3 : 6);
 
-  if (warp == N_CONSUMER_WARPS) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp >= N_CONSUMER_WARPS) {
+    // ===================== TMA producer: every item's k-blocks in item order =====================
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == N_CONSUMER_WARPS && lane == 0) {
       int s = 0;
       uint32_t ph = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -269,7 +286,8 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       }
     }
   } else {
-    // ===================== consumers: MMA, then the epilogue of the warpgroup's 64 rows =====================
+    // ===================== consumers: ping-pong warpgroups, each the MMAs and then the epilogue of its own items =====================
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2, wi = warp & 3;
     const uint32_t smem0 = smem_u32(smem);
     // K-major: SBO = 8 rows * 128 B; MN-major: LBO = stride between 64-wide MN slabs, SBO = 8 k-rows
@@ -280,31 +298,50 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     float* stage_tile = epi_buf + wg * (EPI_WG_BYTES / 4);
     float* stg = stage_tile + wi * 512;                      // this warp's 2 KB tile (after the staging tile has been read)
     const bool use_cs = p.epi.colsum != nullptr && !p.epi.atomic;
-    const int ctid = threadIdx.x;
-    const bool prof = p.prof != nullptr && warp == 0 && lane == 0;
-    int cs_n0 = -1;   // n-tile the shared column-sum accumulator currently holds
-    int s = 0;
+    float* cs_wg = cs_buf + 128 * wg;                        // this warpgroup's column-sum accumulator
+    const int ctid = threadIdx.x & 127;
+    const bool prof = p.prof != nullptr && wi == 0 && lane == 0;
+    const int po = 8 * wg;                                   // this warpgroup's prof slots
+    int cs_n0 = -1;   // n-tile the column-sum accumulator currently holds
+    int s = 0;        // ring position (stage, phase) of the next k-block, over every item of the CTA
     uint32_t ph = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    // item j of the CTA: items of both warpgroups are walked so that the ring position stays in step with the producer
+    for (int j = 0; blockIdx.x + j * gridDim.x < n_items; ++j) {
+      const int item = blockIdx.x + j * gridDim.x;
       const int ks = item % p.k_slices;
       const int t = item / p.k_slices;
       const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * BM;
       const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
+      if ((j & 1) != wg) {                                   // the other warpgroup's item: skip its stages
+        for (int kb = kb0; kb < kb1; ++kb)
+          if (++s == stages) { s = 0; ph ^= 1; }
+        continue;
+      }
       if (use_cs && n0 != cs_n0) {
-        if (cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 32 * N_CONSUMER_WARPS, 1);
+        if (cs_n0 >= 0) colsum_flush(cs_wg, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 128, 2 + wg);
         cs_n0 = n0;
       }
-      float acc[BN / 2];
+      float acc[2][BN / 2];                                  // rows 0-63 and 64-127 of the tile
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.0f;
+      // Wait for this warpgroup's turn: the other one has issued every MMA of item j-1.  Besides keeping the tensor cores
+      // with one warpgroup at a time, this is what makes the parity waits on the shared ring safe: every full-barrier
+      // phase before this item's k-blocks has completed, so a stage cannot be seen one phase early.
+      if (j > 0) {
+        NRW_PROF_T0(prof);
+        named_bar_sync(BAR_TURN + wg, 256);
+        NRW_PROF_ADD(prof, 3 + po);
+      }
       int prev_s = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         {
           NRW_PROF_T0(prof);
           mbar_wait(bar_full + 8 * s, ph);
-          NRW_PROF_ADD(prof, 1);
+          NRW_PROF_ADD(prof, 1 + po);
         }
-        const uint32_t sa = smem0 + s * stage_bytes + wg * WG_A;
+        const uint32_t sa = smem0 + s * stage_bytes;
         const uint32_t sb = smem0 + s * stage_bytes + P * A_TILE;
         wgmma_fence();
         for (int pr = 0; pr < n_prod; ++pr) {
@@ -314,67 +351,78 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
           const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
 #pragma unroll
           for (int k = 0; k < BK / 16; ++k)
-            wgmma_bf16<BN, MN_MAJOR, MN_MAJOR>(acc, da + ((k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)                  // 64-row half h: K-major rows at +8 KB, or the second MN-major slab
+              wgmma_bf16<BN, MN_MAJOR, MN_MAJOR>(acc[h], da + ((h * WG_A + k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
         }
         wgmma_commit();
-        acc_fence(acc);
+        acc_fence(acc[0]);
+        acc_fence(acc[1]);
         if (prev_s >= 0) {                                // the previous stage's MMAs have completed: hand it back
           wgmma_wait<1>();
-          acc_fence(acc);
+          acc_fence(acc[0]);
+          acc_fence(acc[1]);
           if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
         }
         prev_s = s;
         if (++s == stages) { s = 0; ph ^= 1; }
       }
+      // every MMA of this item is issued: the other warpgroup's main loop may start (if the CTA has an item j+1)
+      if (item + gridDim.x < n_items) named_bar_arrive(BAR_TURN + (wg ^ 1), 256);
       wgmma_wait<0>();
-      acc_fence(acc);
+      acc_fence(acc[0]);
+      acc_fence(acc[1]);
       if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
       // (an empty k-slice accumulates nothing and stores nothing)
       if (kb1 <= kb0) continue;
       NRW_PROF_T0(prof);
-      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6], 1ull);
-      // ---- epilogue: 32 columns at a time through the warpgroup's staging tile.  Fragment of warp wi: acc[4j + {0,1}] = row
-      // 16 wi + lane / 4, columns 8 j + 2 (lane % 4) + {0,1}; acc[4j + {2,3}] = the same columns of row + 8.  After the barrier warp
-      // wi takes rows 32 (wi & 1) .. +31 (row = lane) and columns 16 (wi >> 1) .. +15 of the 32: the chunk layout of epi_chunk16. ----
+      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6 + po], 1ull);
+      // ---- epilogue, per 64-row half h: 32 columns at a time through the warpgroup's staging tile.  Fragment of warp wi:
+      // acc[h][4j + {0,1}] = row 64 h + 16 wi + lane / 4, columns 8 j + 2 (lane % 4) + {0,1}; acc[h][4j + {2,3}] = the same columns
+      // of row + 8.  After the barrier warp wi takes rows 64 h + 32 (wi & 1) .. +31 (row = lane) and columns 16 (wi >> 1) .. +15
+      // of the 32: the chunk layout of epi_chunk16. ----
       const int r0 = 16 * wi + (lane >> 2), c0 = 2 * (lane & 3);
       const int qq = wi & 1, cc = wi >> 1;
-      const int m0w = m0 + 64 * wg + 32 * qq;
-      float hacc[4] = {0.0f, 0.0f, 0.0f, 0.0f};     // FWD_HEAD: this lane's rows of the fused SDF-head dot product
       const int n_cp = (min(BN, p.N - n0) + 31) / 32;
 #pragma unroll
-      for (int cp = 0; cp < BN / 32; ++cp) {
-        if (cp >= n_cp) break;                       // warpgroup-uniform
+      for (int h = 0; h < 2; ++h) {
+        const int m0w = m0 + 64 * h + 32 * qq;
+        float hacc[4] = {0.0f, 0.0f, 0.0f, 0.0f};   // FWD_HEAD: this lane's rows of the fused SDF-head dot product
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = 4 * cp + jj;
-          *reinterpret_cast<float2*>(stage_tile + r0 * EPI_LD + 8 * jj + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(stage_tile + (r0 + 8) * EPI_LD + 8 * jj + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-        named_bar_sync(2 + wg, 128);
-        float v[16];
-        const float* src = stage_tile + (32 * qq + lane) * EPI_LD + 16 * cc;
+        for (int cp = 0; cp < BN / 32; ++cp) {
+          if (cp >= n_cp) break;                     // warpgroup-uniform
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 t4 = *reinterpret_cast<const float4*>(src + 4 * i);
-          v[4 * i] = t4.x; v[4 * i + 1] = t4.y; v[4 * i + 2] = t4.z; v[4 * i + 3] = t4.w;
+          for (int jj = 0; jj < 4; ++jj) {
+            const int jf = 4 * cp + jj;
+            *reinterpret_cast<float2*>(stage_tile + r0 * EPI_LD + 8 * jj + c0) = make_float2(acc[h][4 * jf], acc[h][4 * jf + 1]);
+            *reinterpret_cast<float2*>(stage_tile + (r0 + 8) * EPI_LD + 8 * jj + c0) = make_float2(acc[h][4 * jf + 2], acc[h][4 * jf + 3]);
+          }
+          named_bar_sync(2 + wg, 128);
+          float v[16];
+          const float* src = stage_tile + (32 * qq + lane) * EPI_LD + 16 * cc;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float4 t4 = *reinterpret_cast<const float4*>(src + 4 * i);
+            v[4 * i] = t4.x; v[4 * i + 1] = t4.y; v[4 * i + 2] = t4.z; v[4 * i + 3] = t4.w;
+          }
+          named_bar_sync(2 + wg, 128);               // the staging tile is free: it holds the warps' 2 KB tiles from here on
+          const int nc = n0 + 32 * cp + 16 * cc;
+          if (nc < p.N && m0w < p.M)                 // warp-uniform
+            epi_fast16<EK>(p.epi, stg, v, m0w, nc, p.M, p.N, lane, use_cs ? cs_wg + 32 * cp + 16 * cc : nullptr, nullptr, 0, hacc);
+          named_bar_sync(2 + wg, 128);
         }
-        named_bar_sync(2 + wg, 128);                 // the staging tile is free: it holds the warps' 2 KB tiles from here on
-        const int nc = n0 + 32 * cp + 16 * cc;
-        if (nc < p.N && m0w < p.M)                   // warp-uniform
-          epi_fast16<EK>(p.epi, stg, v, m0w, nc, p.M, p.N, lane, use_cs ? cs_buf + 32 * cp + 16 * cc : nullptr, nullptr, 0, hacc);
-        named_bar_sync(2 + wg, 128);
+        if (EK == EK_FWD_HEAD && (lane & 3) == 0) { // partial[row][slot], slot = n-tile * 2 + column class: plain stores
+          const int slot = (n0 / BN) * 2 + cc;
+#pragma unroll
+          for (int it = 0; it < 4; ++it) {
+            const int row = m0w + it * 8 + (lane >> 2);
+            if (row < p.M) p.epi.head_partial[(long long)row * 8 + slot] = hacc[it];
+          }
+        }
       }
-      if (EK == EK_FWD_HEAD && (lane & 3) == 0) {   // partial[row][slot], slot = n-tile * 2 + column class: plain stores
-        const int slot = (n0 / BN) * 2 + cc;
-#pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          const int row = m0w + it * 8 + (lane >> 2);
-          if (row < p.M) p.epi.head_partial[(long long)row * 8 + slot] = hacc[it];
-        }
-      }
-      NRW_PROF_ADD(prof, 4);
+      NRW_PROF_ADD(prof, 4 + po);
     }
-    if (use_cs && cs_n0 >= 0) colsum_flush(cs_buf, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 32 * N_CONSUMER_WARPS, 1);
+    if (use_cs && cs_n0 >= 0) colsum_flush(cs_wg, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 128, 2 + wg);
   }
   __syncthreads();
   if (p.prof && threadIdx.x == 0) atomicAdd(&p.prof[blockIdx.x * 16 + 5], (unsigned long long)(clock64() - t_kernel0));
@@ -560,7 +608,7 @@ static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
   const int dev = current_device();
   if (!n_sm_dev[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm_dev[dev], cudaDevAttrMultiProcessorCount, dev));
   const int n_sm = n_sm_dev[dev];
-  // 128 x 128 tiles (two m64n128 warpgroups): with two operand planes that is 64 KB per k-block and 3 TMA stages
+  // 128 x 128 tiles (one warpgroup, two m64n128 halves): with two operand planes that is 64 KB per k-block and 3 TMA stages
   const int BN = g.N <= 64 ? 64 : 128;
   TcParams p;
   memset(&p, 0, sizeof(p));
