@@ -263,6 +263,19 @@ NRW_API int nrw_grid_points_sparse(const int16_t* leaves, long long n_leaves, in
 NRW_API int nrw_threshold_compact(const float* sdf, const float* xyz /*[n,3]*/, long long n, float threshold, float* out,
                                   int64_t* count, void* scratch, void* stream);
 
+/* ---- masked marching cubes (the mesh step of utils/visualization.py::extract_mesh; rules in csrc/mcubes.cu) -------------
+ * vol: contiguous fp32 [d0,d1,d2] (C order), every d >= 2; mask: uint8 [d0,d1,d2] or NULL, cell (i,j,k) is meshed only
+ * when mask[i+1,j+1,k+1] != 0 (and its 8 corners are finite).  nrw_mc_count writes counts (device int64[2]) = {n_verts,
+ * n_faces} and fills scratch (nrw_mc_scratch_bytes, 256-byte aligned); nrw_mc_emit, given the same volume, level, mask and
+ * scratch and the two counts read back by the caller, writes verts fp32 [n_verts,3] (index coordinates, axis 0 first),
+ * normals fp32 [n_verts,3] and faces int32 [n_faces,3].  n_verts must be <= INT32_MAX.  nrw_mc_scratch_bytes returns a
+ * negative nrw_status for a dimension below 2. */
+NRW_API long long nrw_mc_scratch_bytes(int d0, int d1, int d2);
+NRW_API int nrw_mc_count(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask /*nullable*/,
+                         void* scratch, long long* counts /*device int64[2]: n_verts, n_faces*/, void* stream);
+NRW_API int nrw_mc_emit(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask, const void* scratch,
+                        long long n_verts, long long n_faces, float* verts, float* normals, int32_t* faces, void* stream);
+
 /* ---- unit-test hooks ---------------------------------------------------------------------- */
 /* D[M,N] = (sum planes of A)[M,K] * (sum planes of B)[N,K]^T from fp32 inputs: splits into planes in
  * scratch (caller-provided, nrw_gemm_test_scratch_bytes) and runs the selected backend. */

@@ -321,6 +321,23 @@ int nrw_grid_points_sparse(const int16_t* leaves, long long n_leaves, int up_tim
   NRW_GUARD_END
 }
 
+long long nrw_mc_scratch_bytes(int d0, int d1, int d2) {
+  NRW_CHECK(d0 >= 2 && d1 >= 2 && d2 >= 2, NRW_ERR_ARG, "nrw_mc_scratch_bytes: every dimension must be >= 2 (got %d x %d x %d)", d0, d1, d2);
+  return mc_scratch_bytes(d0, d1, d2);
+}
+int nrw_mc_count(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask, void* scratch, long long* counts,
+                 void* stream) {
+  NRW_GUARD_BEGIN
+  return mc_count(vol, d0, d1, d2, level, mask, scratch, reinterpret_cast<int64_t*>(counts), S(stream));
+  NRW_GUARD_END
+}
+int nrw_mc_emit(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask, const void* scratch, long long n_verts,
+                long long n_faces, float* verts, float* normals, int32_t* faces, void* stream) {
+  NRW_GUARD_BEGIN
+  return mc_emit(vol, d0, d1, d2, level, mask, scratch, n_verts, n_faces, verts, normals, faces, S(stream));
+  NRW_GUARD_END
+}
+
 long long nrw_gemm_test_scratch_bytes(int M, int N, int K) {
   const long long a = round_up((long long)M * K, 512), b = round_up((long long)N * K, 512);
   return (a + b) * 3 * 2 + 4096;

@@ -71,7 +71,7 @@ __global__ void __launch_bounds__(CB) thresh_count_kernel(const float* __restric
 }
 
 // ---- pass 2: exclusive scan of the block counts (one block), total -> n_valid[0] ----------------------------------
-__global__ void __launch_bounds__(1024) scan_counts_kernel(int32_t* __restrict__ counts, int n_blocks, int64_t base,
+__global__ void __launch_bounds__(1024) scan_counts_kernel(const int32_t* __restrict__ counts, int n_blocks, int64_t base,
                                                            int64_t* __restrict__ block_offsets, int64_t* __restrict__ total) {
   __shared__ long long wsum[32];
   __shared__ long long carry_s;
@@ -148,6 +148,13 @@ __global__ void __launch_bounds__(CB) thresh_scatter_kernel(const float* __restr
   if (!keep) return;
   const long long dst = block_offsets[blockIdx.x] + off;
   out[dst * 3] = xyz[i * 3]; out[dst * 3 + 1] = xyz[i * 3 + 1]; out[dst * 3 + 2] = xyz[i * 3 + 2];
+}
+
+// exclusive scan of n int32 counts -> int64 offsets, total -> *total (device); also used by marching cubes (mcubes.cu)
+int scan_counts(const int32_t* counts, int n, int64_t* offsets, int64_t* total, cudaStream_t s) {
+  scan_counts_kernel<<<1, 1024, 0, s>>>(counts, n, 0, offsets, total);
+  NRW_LAUNCH_OK();
+  return NRW_OK;
 }
 
 static inline long long align256(long long x) { return (x + 255) / 256 * 256; }

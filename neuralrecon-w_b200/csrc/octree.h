@@ -38,4 +38,14 @@ int grid_points_dense(int dim, const float lo[3], const float hi[3], long long i
 int grid_points_sparse(const int16_t* leaves, long long n_leaves, int up, float voxel, const float vol_origin[3],
                        const float scene_origin[3], float scene_radius, long long i0, long long n, float* xyz_sfm,
                        float* xyz_train, cudaStream_t s);
+int scan_counts(const int32_t* counts, int n, int64_t* offsets, int64_t* total, cudaStream_t s);
+}  // namespace nrw
+
+// masked marching cubes (mcubes.cu)
+namespace nrw {
+long long mc_scratch_bytes(int d0, int d1, int d2);
+int mc_count(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask, void* scratch, int64_t* counts,
+             cudaStream_t s);
+int mc_emit(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask, const void* scratch, long long n_verts,
+            long long n_faces, float* verts, float* normals, int32_t* faces, cudaStream_t s);
 }  // namespace nrw

@@ -101,6 +101,10 @@ def lib():
     L.nrw_grid_points_dense.argtypes = [i32, C.POINTER(f32), C.POINTER(f32), ll, ll, vp, vp]
     L.nrw_grid_points_sparse.argtypes = [vp, ll, i32, f32, C.POINTER(f32), C.POINTER(f32), f32, ll, ll, vp, vp, vp]
     L.nrw_threshold_compact.argtypes = [vp, vp, ll, f32, vp, vp, vp, vp]
+    L.nrw_mc_scratch_bytes.restype = ll
+    L.nrw_mc_scratch_bytes.argtypes = [i32, i32, i32]
+    L.nrw_mc_count.argtypes = [vp, i32, i32, i32, f32, vp, vp, vp, vp]
+    L.nrw_mc_emit.argtypes = [vp, i32, i32, i32, f32, vp, vp, ll, ll, vp, vp, vp, vp]
     L.nrw_gemm_test_scratch_bytes.restype = ll
     L.nrw_gemm_test_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_gemm_test.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp]
@@ -119,7 +123,8 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_gemm_test_scratch_bytes", "nrw_gemm_test", "nrw_launch_count", "nrw_debug_gemm_profile",
            "nrw_gemm_timing", "nrw_ctx_set_backward_planes", "nrw_octree_build_scratch_bytes", "nrw_octree_build",
            "nrw_grad_sumsq", "nrw_adam_clip_step", "nrw_boundary_samples", "nrw_compact_scratch_bytes", "nrw_raycache_gather",
-           "nrw_grid_points_dense", "nrw_grid_points_sparse", "nrw_threshold_compact", "nrw_ctx_set_backward_gate_planes"]
+           "nrw_grid_points_dense", "nrw_grid_points_sparse", "nrw_threshold_compact", "nrw_ctx_set_backward_gate_planes",
+           "nrw_mc_scratch_bytes", "nrw_mc_count", "nrw_mc_emit"]
 
 
 def check(status, what=""):

@@ -5,9 +5,13 @@ Mirrors the SDF half of utils/visualization.py::extract_mesh (lines 36-107) and 
 chunk back (`.cpu()` per chunk), all-gathers and scatters into a dense volume on the host.  Here the lattice points are
 GENERATED on the device chunk by chunk (nrw_grid_points_dense / nrw_grid_points_sparse) straight into the SDF query
 (nrw_sdf_query), ranks take the contiguous slices of get_local_split (utils/visualization.py:27-35) and one
-all_gather joins them; the dense volume, the validity mask and the scatter stay on the GPU.  Marching cubes
-itself (skimage.measure.marching_cubes) and trimesh export are host-side post-processing and out of scope (DESIGN 8):
-`sdf_volume` / `sparse_sdf_volume` return exactly the arrays the reference hands to marching_cubes."""
+all_gather joins them; the dense volume, the validity mask and the scatter stay on the GPU.  `sdf_volume` /
+`sparse_sdf_volume` return exactly the arrays the reference hands to skimage.measure.marching_cubes.
+
+`marching_cubes` is this library's own masked marching cubes on the device (csrc/mcubes.cu states its rules; it does not
+reproduce skimage's triangulation), and `extract_mesh` is a drop-in for utils/visualization.py::extract_mesh that returns
+a `Mesh` whose `export(path)` writes binary PLY, so neither skimage nor trimesh is needed."""
+import os
 import ctypes as C
 
 import numpy as np
@@ -153,17 +157,184 @@ def sparse_sdf_volume(renderer, grid, chunk=1 << 20, sdf_fn=None):
     outside the lattice; mask_dense bool CUDA - a cell is valid iff all 8 of its corners are lattice points)."""
     res = sparse_candidates(renderer, grid, chunk=chunk, sdf_fn=sdf_fn)
     leaves, up, dim = grid["leaves"].to(torch.int64), int(grid["up_times"]), int(grid["dim"])
-    dev = leaves.device
-    k = torch.arange(up, device=dev)
+    k = torch.arange(up, device=leaves.device)
     kern = torch.stack(torch.meshgrid(k, k, k, indexing="ij"), -1).reshape(-1, 3)
     ind = (leaves[:, None, :] * up + kern[None, :, :]).reshape(-1, 3)          # ind = round((xyz - vol_origin)/voxel)
+    return _scatter_volume(ind, res["sdf"], dim)
+
+
+def _scatter_volume(ind, sdf, dim):
+    """utils/visualization.py:98-116: SDF values at lattice indices ind [n,3] -> (dense volume, ones elsewhere; mask)."""
+    dev = ind.device
     sdf_dense = torch.ones(dim, dim, dim, dtype=torch.float32, device=dev)
-    sdf_dense[ind[:, 0], ind[:, 1], ind[:, 2]] = res["sdf"]
+    sdf_dense[ind[:, 0], ind[:, 1], ind[:, 2]] = sdf
     m = torch.zeros(dim, dim, dim, dtype=torch.bool, device=dev)
     m[ind[:, 0], ind[:, 1], ind[:, 2]] = True
     # a marching-cubes cell (i, j, k) uses the corners (i - a, j - b, k - c), a, b, c in {0, 1} (wrap-around as torch.roll)
     valid = m.clone()
     for shift in ((1, 0, 0), (0, 1, 0), (0, 0, 1), (1, 1, 0), (1, 0, 1), (0, 1, 1), (1, 1, 1)):
         valid &= torch.roll(m, shifts=shift, dims=(0, 1, 2))
-    m = valid
-    return sdf_dense, m
+    return sdf_dense, valid
+
+
+def marching_cubes(volume, level=0.0, mask=None):
+    """Masked marching cubes of a CUDA fp32 volume [d0,d1,d2] (csrc/mcubes.cu): -> (verts fp32 [V,3] in index
+    coordinates, faces int32 [F,3], normals fp32 [V,3]), CUDA tensors.  With `mask` (bool or uint8, same shape) cell
+    (i,j,k) is meshed only when mask[i+1,j+1,k+1] is set, so `marching_cubes(*sparse_sdf_volume(r, grid))` works as is.
+    One host read (the two counts) between the count and emit passes."""
+    L = _lib.lib()
+    if not (torch.is_tensor(volume) and volume.is_cuda and volume.dim() == 3):
+        raise NrwError("marching_cubes: volume must be a 3-D CUDA tensor")
+    if min(volume.shape) < 2:
+        raise NrwError(f"marching_cubes: every dimension must be >= 2 (got {tuple(volume.shape)})")
+    vol = volume.to(torch.float32).contiguous()
+    d0, d1, d2 = (int(x) for x in vol.shape)
+    m = None
+    if mask is not None:
+        if tuple(mask.shape) != tuple(vol.shape) or mask.device != vol.device:
+            raise NrwError("marching_cubes: mask must have the volume's shape and device")
+        m = (mask != 0).to(torch.uint8).contiguous()
+    sb = L.nrw_mc_scratch_bytes(d0, d1, d2)
+    if sb < 0:
+        check(sb, "nrw_mc_scratch_bytes")
+    scratch = torch.empty(sb + 256, dtype=torch.uint8, device=vol.device)
+    sp = C.c_void_p((scratch.data_ptr() + 255) // 256 * 256)
+    counts = torch.empty(2, dtype=torch.int64, device=vol.device)
+    lvl = float(level)
+    check(L.nrw_mc_count(ptr(vol), d0, d1, d2, lvl, ptr(m), sp, ptr(counts), stream_ptr()), "nrw_mc_count")
+    nv, nf = counts.tolist()
+    verts = torch.empty(nv, 3, dtype=torch.float32, device=vol.device)
+    normals = torch.empty(nv, 3, dtype=torch.float32, device=vol.device)
+    faces = torch.empty(nf, 3, dtype=torch.int32, device=vol.device)
+    check(L.nrw_mc_emit(ptr(vol), d0, d1, d2, lvl, ptr(m), sp, nv, nf, ptr(verts), ptr(normals), ptr(faces), stream_ptr()),
+          "nrw_mc_emit")
+    return verts, faces, normals
+
+
+class Mesh:
+    """The slice of trimesh.Trimesh that extract_mesh's callers use: vertices float64 [V,3], faces int64 [F,3],
+    vertex_normals float32 [V,3], vertex_colors uint8 [V,3] or None (numpy), and export(path)."""
+
+    def __init__(self, vertices, faces, vertex_normals, vertex_colors=None):
+        self.vertices = np.asarray(vertices)
+        self.faces = np.asarray(faces, dtype=np.int64)
+        self.vertex_normals = np.asarray(vertex_normals)
+        self.vertex_colors = None if vertex_colors is None else np.asarray(vertex_colors, dtype=np.uint8)
+
+    def export(self, path):
+        """Binary little-endian PLY: vertex x y z nx ny nz (float32) [red green blue (uchar)], face list uchar int."""
+        if os.path.splitext(str(path))[1].lower() != ".ply":
+            raise NrwError(f"Mesh.export: only .ply is supported (got {path})")
+        write_ply(path, self.vertices, self.faces, self.vertex_normals, self.vertex_colors)
+
+
+def write_ply(path, vertices, faces, normals, colors=None):
+    n, f = len(vertices), len(faces)
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+    if colors is not None:
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    v = np.empty(n, dtype=fields)
+    for c, name in enumerate("xyz"):
+        v[name] = vertices[:, c]
+        v["n" + name] = normals[:, c]
+    if colors is not None:
+        for c, name in enumerate(("red", "green", "blue")):
+            v[name] = colors[:, c]
+    fc = np.empty(f, dtype=[("n", "u1"), ("i", "<i4", (3,))])
+    fc["n"] = 3
+    fc["i"] = faces
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {n}"]
+    head += [f"property float {name}" for name in ("x", "y", "z", "nx", "ny", "nz")]
+    if colors is not None:
+        head += [f"property uchar {name}" for name in ("red", "green", "blue")]
+    head += [f"element face {f}", "property list uchar int vertex_indices", "end_header"]
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(head) + "\n").encode("ascii"))
+        fh.write(v.tobytes())
+        fh.write(fc.tobytes())
+
+
+def read_ply(path):
+    """Inverse of write_ply (binary little-endian, the layout above) -> dict of numpy arrays."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    end = data.index(b"end_header\n") + len(b"end_header\n")
+    head = data[:end].decode("ascii").split("\n")
+    nv = int([h for h in head if h.startswith("element vertex")][0].split()[-1])
+    nf = int([h for h in head if h.startswith("element face")][0].split()[-1])
+    props = [h.split()[-1] for h in head if h.startswith("property ") and not h.startswith("property list")]
+    fields = [(p, "<f4" if p in ("x", "y", "z", "nx", "ny", "nz") else "u1") for p in props]
+    v = np.frombuffer(data, dtype=fields, count=nv, offset=end)
+    fc = np.frombuffer(data, dtype=[("n", "u1"), ("i", "<i4", (3,))], count=nf, offset=end + v.nbytes)
+    assert end + v.nbytes + fc.nbytes == len(data) and (fc["n"] == 3).all()
+    out = {"vertices": np.stack([v["x"], v["y"], v["z"]], 1), "normals": np.stack([v["nx"], v["ny"], v["nz"]], 1),
+           "faces": fc["i"].astype(np.int64)}
+    out["colors"] = np.stack([v["red"], v["green"], v["blue"]], 1) if "red" in props else None
+    return out
+
+
+def _sdf_at(renderer, xyz, chunk):
+    """renderer.sdf at training-coordinate points xyz [n,3] (CUDA), rank slices + all_gather as the reference."""
+    n = xyz.shape[0]
+    world, rank = _world()
+    a, b, per = _local_range(n, world, rank)
+    local = torch.empty(max(b - a, 0), dtype=torch.float32, device=xyz.device)
+    with torch.no_grad():
+        for i in range(a, b, chunk):
+            m = min(chunk, b - i)
+            local[i - a:i - a + m] = renderer.sdf(xyz[i:i + m].reshape(-1, 1, 3)).reshape(-1)
+    return _gather_slices(local, per, n, world)
+
+
+def extract_mesh(dim, chunk, scene_radius, scene_origin, origin=None, radius=1.0, with_color=False, embedding_a=None,
+                 chunk_rgb=256, sparse_data=None, renderer=None):
+    """Drop-in for utils/visualization.py::extract_mesh (same signature): SDF volume, marching cubes and vertex colours
+    on the GPU; rank 0 returns a `Mesh` (world coordinates), other ranks None.  `sparse_data` is either the reference's
+    dict (sparse_vol [n,3] SfM points, voxel_size, dim, vol_origin) or the one gen_grid_spc returns (leaves, ...).
+    Colours: renderer.rgb at the training-coordinate vertices, direction (0,0,1), stored as uint8 clamp(round(255 rgb))."""
+    if origin is None:
+        origin = [0, 0, 0]
+    dev = next(renderer.neuconw.parameters()).device
+    if sparse_data is None:
+        vol, vol_origin, voxel_size = sdf_volume(renderer, dim, origin=origin, radius=radius, chunk=chunk)
+        mask = None
+        to_train = lambda v: v * voxel_size + vol_origin                       # float32 * float -> float32, + float64
+        to_world = lambda v: v * scene_radius + np.array(scene_origin)
+    else:
+        # utils/visualization.py:57-65: training-coordinate origin and voxel size of the sparse lattice
+        vol_origin_sfm = torch.from_numpy(np.array(sparse_data["vol_origin"])).float()
+        so = torch.from_numpy(np.array(scene_origin)).float()
+        vol_origin = ((vol_origin_sfm - so) / scene_radius).numpy()
+        voxel_size = sparse_data["voxel_size"] / scene_radius
+        if "leaves" in sparse_data:
+            vol, mask = sparse_sdf_volume(renderer, sparse_data, chunk=chunk)
+        else:
+            sv = torch.as_tensor(sparse_data["sparse_vol"]).float()
+            ind = torch.round((sv - vol_origin_sfm) / sparse_data["voxel_size"]).long().to(dev)
+            xyz = ((sv - so) / scene_radius).to(dev)
+            vol, mask = _scatter_volume(ind, _sdf_at(renderer, xyz, chunk), int(sparse_data["dim"]))
+        so_np = so.numpy()
+        to_train = lambda v: v * voxel_size + vol_origin                       # float32 throughout
+        to_world = lambda v: v * scene_radius + so_np
+    verts, faces, normals = marching_cubes(vol, 0.0, mask)
+    verts_t = to_train(verts.cpu().numpy())
+    verts_w = to_world(verts_t)
+    colors = None
+    if with_color:
+        world, rank = _world()
+        n = verts_t.shape[0]
+        a, b, per = _local_range(n, world, rank)
+        pts = torch.from_numpy(np.ascontiguousarray(verts_t)).float().to(dev)
+        emb = embedding_a.detach().reshape(1, -1).to(dev)
+        local = torch.empty(max(b - a, 0), 3, dtype=torch.float32, device=dev)
+        with torch.no_grad():
+            for i in range(a, b, chunk_rgb):
+                m = min(chunk_rgb, b - i)
+                d = torch.zeros(m, 1, 3, dtype=torch.float32, device=dev)
+                d[:, :, 2] = 1
+                local[i - a:i - a + m] = renderer.rgb(pts[i:i + m].reshape(-1, 1, 3), d, emb.repeat(m, 1).reshape(m, 1, -1))
+        rgb = _gather_slices(local.reshape(-1), per * 3, n * 3, world).reshape(n, 3)
+        colors = torch.round(rgb * 255).clamp(0, 255).to(torch.uint8).cpu().numpy()
+    if _world()[1] != 0:
+        return None
+    return Mesh(verts_w, faces.cpu().numpy(), normals.cpu().numpy(), colors)
