@@ -75,6 +75,7 @@ int nrw_ctx_set_backward_planes(nrw_ctx* ctx, int n) {
 int nrw_ctx_set_backward_gate_planes(nrw_ctx* ctx, int n) {
   NRW_GUARD_BEGIN
   NRW_CHECK(ctx != nullptr && n >= 0 && n <= ctx->n_planes, NRW_ERR_ARG, "set_backward_gate_planes: n=%d outside 0..n_planes", n);
+  NRW_CHECK(!ctx->bound, NRW_ERR_STATE, "set_backward_gate_planes: call before nrw_ctx_bind (it changes the workspace layout)");
   ctx->bwd_gate_planes = n;
   return NRW_OK;
   NRW_GUARD_END

@@ -1,8 +1,8 @@
 // Chunked orchestration of the per-ray hot path: sampler -> background NeRF -> SDF value/normal ->
 // colour net -> compositing, and the hand-derived backward of all of it (SURVEY.md 9.2/9.3).
 // Every dense layer is one tensor-core GEMM launch with a fused epilogue; chunks of `Mc` samples keep the
-// inter-layer activations L2-resident.  Backward recomputes the forward of a chunk into the workspace
-// and immediately consumes it, so memory is O(chunk) instead of O(batch).
+// inter-layer activations L2-resident.  Backward consumes a chunk's forward from its slot; chunks that found no slot of
+// their own are recomputed into the workspace and consumed at once, so memory is O(slots x chunk), not O(batch).
 #include <stdlib.h>
 
 #include "engine.h"
@@ -36,14 +36,25 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
                   int n_slots_nerf) {
   const int P = c.n_planes;
   const long long M = Mc;
+  // In 'mixed' nothing after a chunk's own forward reads the lo plane of its activations: the backward GEMMs, gates, ReLU
+  // masks and heads all run on the hi plane.  So slots 1.. keep only the hi plane of each two-plane tensor and point their
+  // plane 1 (pstride = lo - hi, negative) at slot 0's lo plane, which every slot shares as scratch.
+  const bool shared_lo = P == 2 && c.bwd_planes == 1 && c.gate_planes() == 1;
+  auto fwd_planes = [&](int slot, const Planes& slot0, int ld) {
+    if (slot == 0 || !shared_lo) return cv.planes(M, ld, P);
+    Planes h = cv.planes(M, ld, 1);
+    if (!cv.dry) h.pstride = slot0.plane(1) - h.p;
+    return h;
+  };
   c.sdf_slots.assign(n_slots_sdf, FwdSdfSlot{});
   c.nerf_slots.assign(n_slots_nerf, FwdNerfSlot{});
   for (int i = 0; i < n_slots_sdf; ++i) {
     FwdSdfSlot& s = c.sdf_slots[i];
+    const FwdSdfSlot& s0 = c.sdf_slots[0];
     s.PTS = cv.f32(M * 3);
-    s.U0 = cv.planes(M, 64, P);
-    for (int l = 1; l <= 8; ++l) s.U[l] = cv.planes(M, 512, P);
-    for (int l = 0; l < 8; ++l) s.G[l] = cv.planes(M, 512, P);
+    s.U0 = fwd_planes(i, s0.U0, 64);
+    for (int l = 1; l <= 8; ++l) s.U[l] = fwd_planes(i, s0.U[l], 512);
+    for (int l = 0; l < 8; ++l) s.G[l] = fwd_planes(i, s0.G[l], 512);
     s.Q[0] = cv.f32(M * 64);
     for (int l = 1; l < 8; ++l) {
       s.Q[l] = nullptr; s.Qh[l] = nullptr;
@@ -51,24 +62,25 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
       else s.Q[l] = cv.f32(M * 512);
     }
     s.Qh[0] = nullptr;
-    s.FEAT = cv.planes(M, 512, P);
+    s.FEAT = fwd_planes(i, s0.FEAT, 512);
     s.c_sdf = cv.f32(M);
     s.HP = cv.f32(M * 8);
     s.c_nrm = cv.f32(M * 3);
-    s.IN1 = cv.planes(M, 640, P);
-    s.H1 = cv.planes(M, 128, P);
-    s.IN2 = cv.planes(M, 192, P);
-    for (int l = 1; l <= 4; ++l) s.X[l] = cv.planes(M, 256, P);
+    s.IN1 = fwd_planes(i, s0.IN1, 640);
+    s.H1 = fwd_planes(i, s0.H1, 128);
+    s.IN2 = fwd_planes(i, s0.IN2, 192);
+    for (int l = 1; l <= 4; ++l) s.X[l] = fwd_planes(i, s0.X[l], 256);
     s.c_rgb = cv.f32(M * 3);
   }
   for (int i = 0; i < n_slots_nerf; ++i) {
     FwdNerfSlot& s = c.nerf_slots[i];
-    s.IN0 = cv.planes(M, 128, P);
+    const FwdNerfSlot& s0 = c.nerf_slots[0];
+    s.IN0 = fwd_planes(i, s0.IN0, 128);
     for (int l = 1; l <= 8; ++l)
-      if (l != 5) s.NH[l] = cv.planes(M, 256, P);
-    s.IN5 = cv.planes(M, 384, P);
-    s.FEATN = cv.planes(M, 384, P);
-    for (int l = 1; l <= 4; ++l) s.AP[l] = cv.planes(M, 128, P);
+      if (l != 5) s.NH[l] = fwd_planes(i, s0.NH[l], 256);
+    s.IN5 = fwd_planes(i, s0.IN5, 384);
+    s.FEATN = fwd_planes(i, s0.FEATN, 384);
+    for (int l = 1; l <= 4; ++l) s.AP[l] = fwd_planes(i, s0.AP[l], 128);
     s.c_density = cv.f32(M);
     s.c_alpha = cv.f32(M);
     s.c_rgbbg = cv.f32(M * 3);
@@ -81,29 +93,30 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
   c.fwd_cached = false;
   c.ge_acc = cv.f32(4);
   if (with_bwd) {
-    c.DQ0 = cv.planes(M, 64, P);
-    c.DQodd = cv.planes(M, 512, P);
-    c.DQeven = cv.planes(M, 512, P);
-    c.DQ4 = cv.planes(M, 512, P);
-    c.DA[0] = cv.planes(M, 512, P);
-    c.DA[1] = cv.planes(M, 512, P);
-    c.DFEAT = cv.planes(M, 512, P);
+    const int PB = c.bwd_planes > 0 ? c.bwd_planes : P;   // the backward writes and reads only its own planes
+    c.DQ0 = cv.planes(M, 64, PB);
+    c.DQodd = cv.planes(M, 512, PB);
+    c.DQeven = cv.planes(M, 512, PB);
+    c.DQ4 = cv.planes(M, 512, PB);
+    c.DA[0] = cv.planes(M, 512, PB);
+    c.DA[1] = cv.planes(M, 512, PB);
+    c.DFEAT = cv.planes(M, 512, PB);
     c.DQ8f = cv.f32(M * 512);
     for (int l = 0; l < 8; ++l) {
       c.DA2[l] = nullptr; c.DA2h[l] = nullptr;
       if (c.aux_bf16) c.DA2h[l] = reinterpret_cast<bf16*>(cv.take(M * 512 * 2));
       else c.DA2[l] = cv.f32(M * 512);
     }
-    c.dX[0] = cv.planes(M, 256, P);
-    c.dX[1] = cv.planes(M, 256, P);
-    c.dH2 = cv.planes(M, 128, P);
-    c.dH1 = cv.planes(M, 128, P);
-    c.dXF = cv.planes(M, 512, P);
-    c.dNA[0] = cv.planes(M, 128, P);
-    c.dNA[1] = cv.planes(M, 128, P);
-    c.dNF = cv.planes(M, 256, P);
-    c.dNH[0] = cv.planes(M, 256, P);
-    c.dNH[1] = cv.planes(M, 256, P);
+    c.dX[0] = cv.planes(M, 256, PB);
+    c.dX[1] = cv.planes(M, 256, PB);
+    c.dH2 = cv.planes(M, 128, PB);
+    c.dH1 = cv.planes(M, 128, PB);
+    c.dXF = cv.planes(M, 512, PB);
+    c.dNA[0] = cv.planes(M, 128, PB);
+    c.dNA[1] = cv.planes(M, 128, PB);
+    c.dNF = cv.planes(M, 256, PB);
+    c.dNH[0] = cv.planes(M, 256, PB);
+    c.dNH[1] = cv.planes(M, 256, PB);
     c.tail = cv.f32(M * 128);
     c.c_dn = cv.f32(M * 3);
     c.c_ddens = cv.f32(M);
@@ -529,8 +542,8 @@ int render_forward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& i
   NRW_CHECK(R <= c.max_rays && T <= c.max_T, NRW_ERR_WORKSPACE, "render: R=%d T=%d exceed bound workspace", R, T);
   NRW_CHECK(c.Mc >= T, NRW_ERR_WORKSPACE, "render: chunk_rows=%d smaller than one ray (%d)", c.Mc, T);
   const bool bg = cfg.n_outside > 0;
-  // keep every chunk's activations for the backward pass when the bound workspace has a slot per chunk
-  const bool cache = c.with_bwd && cdiv(R, c.Mc / S) <= c.n_slots_sdf && (!bg || cdiv(R, c.Mc / T) <= c.n_slots_nerf);
+  // chunk ci keeps its activations for the backward pass in slot min(ci, k - 1) of the k bound slots: chunks 0 .. k-2
+  // stay resident, and so does the last chunk, which is the last one written into slot k - 1 (render_backward)
   c.fwd_cached = false;
   if (bg) {
     NRW_TRY(launch_merge_sorted(R, S, cfg.n_outside, io.z_vals, io.z_out, io.sv_z_feed, s));
@@ -538,7 +551,7 @@ int render_forward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& i
     for (int r0 = 0, ci = 0; r0 < R; r0 += rc, ++ci) {
       const int nr = (R - r0) < rc ? (R - r0) : rc;
       const int M = nr * T;
-      c.use_nerf_slot(cache ? ci : 0);
+      c.use_nerf_slot(ci < c.n_slots_nerf ? ci : c.n_slots_nerf - 1);
       NRW_TRY(nerf_chunk_forward(c, M, io.o + r0 * 3, io.d + r0 * 3, io.sv_z_feed + (long long)r0 * T,
                                  io.sample_dist + r0, nullptr, io.a_emb + (long long)r0 * c.n_a, T, T, s));
       NRW_CUDA_OK(cudaMemcpyAsync(io.sv_bg_alpha + (long long)r0 * T, c.c_alpha, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
@@ -549,7 +562,7 @@ int render_forward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& i
   for (int r0 = 0, ci = 0; r0 < R; r0 += rc, ++ci) {
     const int nr = (R - r0) < rc ? (R - r0) : rc;
     const int M = nr * S;
-    c.use_sdf_slot(cache ? ci : 0);
+    c.use_sdf_slot(ci < c.n_slots_sdf ? ci : c.n_slots_sdf - 1);
     NRW_TRY(launch_points(io.o + r0 * 3, io.d + r0 * 3, io.z_vals + (long long)r0 * S, io.sample_dist + r0, nr, S, 1, c.PTS, s));
     NRW_TRY(sdf_chunk_forward(c, M, c.PTS, true, true, s));
     NRW_TRY(color_chunk_forward(c, M, c.PTS, io.d + r0 * 3, io.a_emb + (long long)r0 * c.n_a, S, s));
@@ -559,9 +572,19 @@ int render_forward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& i
   }
   NRW_TRY(composite_forward(cfg, io, io.sv_sdf, io.gradients, io.sv_rgb, bg ? io.sv_bg_alpha : nullptr,
                             bg ? io.sv_bg_rgb : nullptr, c.ge_acc, s));
-  c.fwd_cached = cache;
+  c.fwd_cached = c.with_bwd;
   c.cached_R = R; c.cached_S = S; c.cached_T = T; c.cached_gen = cfg.reserved0;
   return NRW_OK;
+}
+
+// The backward visits the n chunks of a pass kept in n_slots slots (render_forward) in this order: the chunks below the
+// last slot, each from its own slot; the last chunk, which the last slot still holds; then the other chunks that shared
+// the last slot, each recomputed there.  With a slot per chunk that is chunk order.  When !cached every chunk is recomputed.
+struct ChunkWalk { int ci, slot; bool resident; };
+static ChunkWalk chunk_walk(int j, int n, int n_slots, bool cached) {
+  const int last = (n < n_slots ? n : n_slots) - 1;
+  const int ci = j < last ? j : j == last ? n - 1 : j - 1;
+  return ChunkWalk{ci, ci < last ? ci : last, cached && (ci == n - 1 || ci < last)};
 }
 
 int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, const nrw_render_grads& g,
@@ -575,28 +598,32 @@ int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& 
   NRW_TRY(composite_backward(cfg, io, g, io.sv_sdf, io.gradients, io.sv_rgb, bg ? io.sv_bg_alpha : nullptr,
                              bg ? io.sv_bg_rgb : nullptr, c.g_dsdf, c.g_dnrm, c.g_drgb, bg ? c.g_dbga : nullptr,
                              bg ? c.g_dbgc : nullptr, g.grad_inv_s, s));
-  // forward activations still resident in per-chunk slots?  otherwise recompute chunk by chunk into slot 0
-  // (the generation stamp guards against a second render_forward having overwritten the slots: ADVICE r1)
+  // do the slots still hold this render's forward?  Otherwise every chunk is recomputed (the generation stamp guards
+  // against a second render_forward having overwritten the slots: ADVICE r1)
   const bool cached = c.fwd_cached && c.cached_R == R && c.cached_S == S && c.cached_T == T && c.cached_gen == cfg.reserved0;
   if (bg) {
-    const int rc = c.Mc / T;
-    for (int r0 = 0, ci = 0; r0 < R; r0 += rc, ++ci) {
+    const int rc = c.Mc / T, n = cdiv(R, rc);
+    for (int j = 0; j < n; ++j) {
+      const ChunkWalk w = chunk_walk(j, n, c.n_slots_nerf, cached);
+      const int r0 = w.ci * rc;
       const int nr = (R - r0) < rc ? (R - r0) : rc;
       const int M = nr * T;
-      c.use_nerf_slot(cached ? ci : 0);
-      if (!cached)
+      c.use_nerf_slot(w.slot);
+      if (!w.resident)
         NRW_TRY(nerf_chunk_forward(c, M, io.o + r0 * 3, io.d + r0 * 3, io.sv_z_feed + (long long)r0 * T,
                                    io.sample_dist + r0, nullptr, io.a_emb + (long long)r0 * c.n_a, T, T, s));
       NRW_TRY(nerf_chunk_backward(c, M, c.g_dbga + (long long)r0 * T, c.g_dbgc + (long long)r0 * T * 3,
                                   g.grad_a_emb + (long long)r0 * c.n_a, nr, T, s));
     }
   }
-  const int rc = c.Mc / S;
-  for (int r0 = 0, ci = 0; r0 < R; r0 += rc, ++ci) {
+  const int rc = c.Mc / S, n = cdiv(R, rc);
+  for (int j = 0; j < n; ++j) {
+    const ChunkWalk w = chunk_walk(j, n, c.n_slots_sdf, cached);
+    const int r0 = w.ci * rc;
     const int nr = (R - r0) < rc ? (R - r0) : rc;
     const int M = nr * S;
-    c.use_sdf_slot(cached ? ci : 0);
-    if (!cached) {
+    c.use_sdf_slot(w.slot);
+    if (!w.resident) {
       NRW_TRY(launch_points(io.o + r0 * 3, io.d + r0 * 3, io.z_vals + (long long)r0 * S, io.sample_dist + r0, nr, S, 1, c.PTS, s));
       NRW_TRY(sdf_chunk_forward(c, M, c.PTS, true, true, s));
       NRW_TRY(color_chunk_forward(c, M, c.PTS, io.d + r0 * 3, io.a_emb + (long long)r0 * c.n_a, S, s));

@@ -101,8 +101,8 @@ class Engine:
     # ---- context / workspace ----------------------------------------------------------------
     def ensure(self, device, max_rays, max_T, with_backward, S=None, chunk_hint=0):
         """(Re)bind the workspace.  With backward enabled, as many chunk slots as the memory budget
-        (NRW_SLOT_BUDGET_GB, default 60 % of free HBM) allows keep their forward activations resident so
-        the backward pass does not recompute the forward (when the HBM holds all chunks of the batch).
+        (NRW_SLOT_BUDGET_GB, default 70 % of free HBM) allows keep their forward activations resident so
+        the backward pass does not recompute the forward of those chunks (NRW_RECOMPUTE=1: one slot each).
 
         Bounds only ever grow.  `max_rays x max_T` sizes the PER-RAY scratch of render / sample; point queries
         (sdf, neuconw_forward, nerf_forward) need chunk buffers only and pass `chunk_hint` (rows they would like one
@@ -136,13 +136,21 @@ class Engine:
                 # last chunk: e.g. 8192 rays x 142 samples = 4.4 chunks of 262144 rows -> 5 chunks of 232,832 rows)
                 n_chunks = -(-(max_rays * max_T) // chunk)
                 balanced = ((-(-max_rays // n_chunks) * max_T + 127) // 128) * 128
+                best = None
                 for cand in ([chunk, balanced] if balanced < chunk else [chunk]):
                     want_sdf = -(-max_rays // max(cand // S_eff, 1))
                     want_nerf = -(-max_rays // max(cand // max_T, 1))
-                    need = self.L.nrw_workspace_bytes(self.ctx, cand, with_backward, max_rays, max_T, want_sdf, want_nerf)
-                    if need <= budget:
-                        chunk, ns_sdf, ns_nerf = cand, want_sdf, want_nerf
-                        break
+                    fits = lambda k_sdf, k_nerf: self.L.nrw_workspace_bytes(
+                        self.ctx, cand, with_backward, max_rays, max_T, k_sdf, k_nerf) <= budget
+                    # as many chunks as fit (the others are recomputed in the backward), SDF slots first: an SDF chunk's
+                    # forward costs more per byte of slot than a NeRF chunk's
+                    k_sdf = next((k for k in range(want_sdf, 0, -1) if fits(k, 1)), 0)
+                    k_nerf = next((k for k in range(want_nerf, 0, -1) if fits(k_sdf, k)), 0)
+                    missing = (want_sdf - k_sdf, want_nerf - k_nerf)
+                    if k_sdf and k_nerf and (best is None or missing < best[0]):
+                        best = (missing, cand, k_sdf, k_nerf)
+                if best is not None:
+                    _, chunk, ns_sdf, ns_nerf = best
             wb = self.L.nrw_workspace_bytes(self.ctx, chunk, with_backward, max_rays, max_T, ns_sdf, ns_nerf)
             self.workspace = torch.empty(wb + 2048, dtype=torch.uint8, device=device)
             pk = (self.packed.data_ptr() + 1023) // 1024 * 1024
