@@ -359,7 +359,7 @@ int nrw_gemm_test(int backend, int n_planes, int mn_major, int k_slices, int M, 
   g.epi.bias = bias; g.epi.act = act; g.epi.out_f32 = D; g.epi.ld_f32 = N; g.epi.atomic = k_slices > 1 ? 1 : 0;
   if (getenv("NRW_GEMM_TEST_LAYER") && !mn_major && k_slices == 1 && N <= K) {
     // tuning: the SDF forward-layer store pattern (fp32 pre-activation + split planes of the activation, written over A)
-    g.epi.out_f32 = nullptr; g.epi.out_pre = D; g.epi.ld_pre = N;
+    g.epi.out_f32 = nullptr; g.epi.out_pre = side_f32(D, N);
     g.epi.out_pl = PA; g.epi.n_planes = n_planes; g.epi.n_store = N;
   }
   return gemm(backend, g, S(stream));

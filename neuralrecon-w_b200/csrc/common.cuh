@@ -52,9 +52,9 @@ static inline long long round_up(long long a, long long b) { return (a + b - 1) 
 // torch.nn.Softplus(beta=100, threshold=20) and its first/second derivatives
 // (reference models/neuconw.py:261; autograd formulas of softplus_backward /
 // softplus_double_backward).
-// MUFU-based forms (ex2 / lg2 / rcp, ~2^-22 relative): the absolute error of softplus is < 4e-9,
+// MUFU-based forms (ex2 / lg2, ~2^-22 relative): the absolute error of softplus is < 4e-9,
 // far below the tensor-core accumulation error of the layer that produced `v`.
-// All three are BRANCH-FREE (a guarded MUFU sequence makes nvcc emit one divergent branch per element,
+// Both are BRANCH-FREE (a guarded MUFU sequence makes nvcc emit one divergent branch per element,
 // which serialises the 32 independent elements a thread owns: measured 130 cycles/element).
 __device__ __forceinline__ float mufu_ex2(float x) {
   float y;
@@ -64,11 +64,6 @@ __device__ __forceinline__ float mufu_ex2(float x) {
 __device__ __forceinline__ float mufu_lg2(float x) {
   float y;
   asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float mufu_rcp(float x) {
-  float y;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 __device__ __forceinline__ float fsel(bool c, float a, float b) {
@@ -82,17 +77,7 @@ __device__ __forceinline__ float softplus100(float v) {
   const float sp = mufu_lg2(1.0f + e) * (0.69314718055994531f * 0.01f);
   return fsel(t > 20.0f, v, sp);
 }
-__device__ __forceinline__ float softplus100_d1(float v) {  // d softplus / dv  (== 1 to 2e-9 above the threshold)
-  const float t = fminf(100.0f * v, 80.0f);
-  return mufu_rcp(1.0f + mufu_ex2(-t * 1.44269504088896341f));
-}
-__device__ __forceinline__ void softplus100_d12(float v, float& d1, float& d2) {
-  const float t = fminf(100.0f * v, 80.0f);
-  const float s = mufu_rcp(1.0f + mufu_ex2(-t * 1.44269504088896341f));
-  d1 = s;
-  d2 = fsel(t > 20.0f, 0.0f, 100.0f * s * (1.0f - s));
-}
-// The same two derivatives from the softplus OUTPUT u = softplus100(v) (what the forward pass keeps as bf16 planes), so
+// Its first and second derivatives from the softplus OUTPUT u = softplus100(v) (what the forward pass keeps as bf16 planes), so
 // the fp32 pre-activation never has to be stored:  exp(-100 u) = 1 / (1 + exp(100 v)) = 1 - sigmoid(100 v), hence
 //   d1 = 1 - exp(-100 u)   (series below 100 u = 0.02: 1 - e cancels),   d2 = 100 d1 (1 - d1) = 100 d1 exp(-100 u).
 // Above the threshold (100 v > 20) the forward stored u = v, so 100 u > 20 reproduces torch's d1 = 1, d2 = 0 branch.
@@ -102,11 +87,6 @@ __device__ __forceinline__ void softplus100_d12_from_u(float u, float& d1, float
   const float ser = x * (1.0f - x * (0.5f - x * 0.16666667f));
   d1 = fsel(x < 0.02f, ser, 1.0f - e);
   d2 = fsel(x > 20.0f, 0.0f, 100.0f * d1 * e);
-}
-__device__ __forceinline__ float softplus100_d2(float v) {  // d2 softplus / dv2
-  float d1, d2;
-  softplus100_d12(v, d1, d2);
-  return d2;
 }
 // accurate form (compositing subtracts two nearby sigmoids: renderer.py:627-632)
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }

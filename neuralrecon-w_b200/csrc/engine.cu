@@ -55,13 +55,9 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
     s.U0 = fwd_planes(i, s0.U0, 64);
     for (int l = 1; l <= 8; ++l) s.U[l] = fwd_planes(i, s0.U[l], 512);
     for (int l = 0; l < 8; ++l) s.G[l] = fwd_planes(i, s0.G[l], 512);
-    s.Q[0] = cv.f32(M * 64);
-    for (int l = 1; l < 8; ++l) {
-      s.Q[l] = nullptr; s.Qh[l] = nullptr;
-      if (c.aux_bf16 && l != 4) s.Qh[l] = reinterpret_cast<bf16*>(cv.take(M * 512 * 2));
-      else s.Q[l] = cv.f32(M * 512);
-    }
-    s.Qh[0] = nullptr;
+    s.Q[0] = side_f32(cv.f32(M * 64), 64);
+    for (int l = 1; l < 8; ++l)   // Q_0 and Q_4 feed the normal in fp32
+      s.Q[l] = c.aux_bf16 && l != 4 ? side_bf16(reinterpret_cast<bf16*>(cv.take(M * 512 * 2)), 512) : side_f32(cv.f32(M * 512), 512);
     s.FEAT = fwd_planes(i, s0.FEAT, 512);
     s.c_sdf = cv.f32(M);
     s.HP = cv.f32(M * 8);
@@ -102,11 +98,8 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
     c.DA[1] = cv.planes(M, 512, PB);
     c.DFEAT = cv.planes(M, 512, PB);
     c.DQ8f = cv.f32(M * 512);
-    for (int l = 0; l < 8; ++l) {
-      c.DA2[l] = nullptr; c.DA2h[l] = nullptr;
-      if (c.aux_bf16) c.DA2h[l] = reinterpret_cast<bf16*>(cv.take(M * 512 * 2));
-      else c.DA2[l] = cv.f32(M * 512);
-    }
+    for (int l = 0; l < 8; ++l)
+      c.DA2[l] = c.aux_bf16 ? side_bf16(reinterpret_cast<bf16*>(cv.take(M * 512 * 2)), 512) : side_f32(cv.f32(M * 512), 512);
     c.dX[0] = cv.planes(M, 256, PB);
     c.dX[1] = cv.planes(M, 256, PB);
     c.dH2 = cv.planes(M, 128, PB);
@@ -237,8 +230,7 @@ int sdf_chunk_forward(nrw_ctx& c, int M, const float* pts, bool need_normal, boo
   const float* b0 = c.f_area + c.pm.heads.sdf_b0;
   // forward-only query (sampler, NeuconWRenderer.sdf, mesh / refresh pipelines): the SDF head is fused into the epilogue of
   // the last layer - u_8 is never written, the head kernel never reads it (tensor-core kernel, M >= 256)
-  static const int no_fused_head = getenv("NRW_FUSED_HEAD") ? !atoi(getenv("NRW_FUSED_HEAD")) : 0;
-  const bool fused_head = !need_normal && !need_feat && M >= 256 && c.backend == NRW_GEMM_TCGEN05 && !no_fused_head;
+  const bool fused_head = !need_normal && !need_feat && M >= 256 && c.backend == NRW_GEMM_TCGEN05;
   // NRW_SDF_FUSED=1: the whole forward-only chain (encoding, 8 layers, head) as ONE kernel with the activations resident in
   // shared memory (gemm_tc.cu::sdf_fused_kernel) - two-plane operands only
   if (fused_head && sdf_fused_enabled(c)) return sdf_fused_query(c, pts, M, c.c_sdf, s);
@@ -264,16 +256,16 @@ int sdf_chunk_forward(nrw_ctx& c, int M, const float* pts, bool need_normal, boo
   if (need_normal) {
     for (int l = 7; l >= 1; --l) {
       Epi e;
-      e.out_pre = c.Q[l]; e.out_pre_h = c.Qh[l]; e.ld_pre = 512;     // exactly one of the two is allocated
+      e.out_pre = c.Q[l];
       gate_from(c, e, l - 1, c.n_planes);
       e.out_pl = c.G[l - 1];
       if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }
       NRW_TRY(mm(c, c.G[l], c.WT(L_SDF0 + l), M, 512, 512, e, s));
     }
     Epi e;
-    e.out_pre = c.Q[0]; e.ld_pre = 64;
+    e.out_pre = c.Q[0];
     NRW_TRY(mm(c, c.G[0], c.WT(L_SDF0), M, 64, 512, e, s));
-    NRW_TRY(launch_sdf_normal(pts, c.Q[0], c.Q[4], M, c.c_nrm, s));
+    NRW_TRY(launch_sdf_normal(pts, c.Q[0].f32(), c.Q[4].f32(), M, c.c_nrm, s));
   }
   return NRW_OK;
 }
@@ -398,9 +390,8 @@ int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, 
     NRW_TRY(mm_dw(c, c.G[l], DQl, M, L_SDF0 + l, s));
     Epi e;
     gate_from(c, e, l, c.gate_planes());
-    e.ld_aux = 512;
-    if (l == 7) { e.aux_q = w0; e.aux_q_bcast = 1; } else { e.aux_q = c.Q[l + 1]; e.aux_q_h = c.Qh[l + 1]; }
-    e.out2 = c.DA2[l]; e.out2_h = c.DA2h[l]; e.ld_out2 = 512;
+    if (l == 7) { e.aux_q = side_f32(w0, 0); e.aux_q_bcast = 1; } else { e.aux_q = c.Q[l + 1]; }
+    e.out2 = c.DA2[l];
     if (l == 3) { e.scale = INV_SQRT2; e.n_store = 473; }
     if (l < 7) e.out_pl = dq_buf(c, l + 1);
     else { e.out_f32 = c.DQ8f; e.ld_f32 = 512; }
@@ -414,7 +405,7 @@ int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, 
     Epi e;
     e.rowvec = d_sdf; e.colvec = w0;
     gate_from(c, e, 7, c.gate_planes());
-    e.aux_add = c.DA2[7]; e.aux_add_h = c.DA2h[7]; e.ld_aux = 512;
+    e.aux_add = c.DA2[7];
     e.out_pl = c.DA[1];
     e.colsum = c.db(L_SDF0 + 7);
     NRW_TRY(mm(c, c.DFEAT, c.WT(L_SDF8F), M, 512, 512, e, s));
@@ -424,7 +415,7 @@ int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, 
     NRW_TRY(mm_dw(c, cur, c.U[l], M, L_SDF0 + l, s));
     Epi e;
     gate_from(c, e, l - 1, c.gate_planes());
-    e.aux_add = c.DA2[l - 1]; e.aux_add_h = c.DA2h[l - 1]; e.ld_aux = 512;
+    e.aux_add = c.DA2[l - 1];
     e.out_pl = c.DA[(l - 1) & 1];
     e.colsum = c.db(L_SDF0 + l - 1);
     if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }

@@ -11,8 +11,7 @@
 struct FwdSdfSlot {
   float* PTS;
   nrw::Planes U0, U[9], G[8], FEAT;
-  float* Q[8];
-  nrw::bf16* Qh[8];     // bf16 twin of Q[l] (l != 0, 4) when the context keeps backward-only side streams in bf16
+  nrw::SideStream Q[8];   // Q_l of the gradient chain ([Mc,64] for l = 0); one bf16 plane for l != 0, 4 when aux_bf16
   float *c_sdf, *c_nrm;
   float* HP;            // [Mc, 8] row partials of the fused SDF head (forward-only queries)
   nrw::Planes IN1, H1, IN2, X[5];
@@ -38,7 +37,7 @@ struct nrw_ctx {
     const FwdSdfSlot& s = sdf_slots[i];
     PTS = s.PTS; U0 = s.U0; FEAT = s.FEAT; c_sdf = s.c_sdf; c_nrm = s.c_nrm; HP = s.HP;
     for (int l = 0; l < 9; ++l) U[l] = s.U[l];
-    for (int l = 0; l < 8; ++l) { G[l] = s.G[l]; Q[l] = s.Q[l]; Qh[l] = s.Qh[l]; }
+    for (int l = 0; l < 8; ++l) { G[l] = s.G[l]; Q[l] = s.Q[l]; }
     IN1 = s.IN1; H1 = s.H1; IN2 = s.IN2; c_rgb = s.c_rgb;
     for (int l = 0; l < 5; ++l) X[l] = s.X[l];
   }
@@ -61,9 +60,7 @@ struct nrw_ctx {
   // ---- chunk workspace (rows = Mc) ----
   float* PTS = nullptr;
   nrw::Planes U0, U[9], G[8], FEAT;
-  float* Q[8] = {nullptr};   // Q[0] is [Mc,64]
-  nrw::bf16* Qh[8] = {nullptr};
-  nrw::bf16* DA2h[8] = {nullptr};
+  nrw::SideStream Q[8];
   bool aux_bf16 = false;     // 'mixed': Q_l (l != 0, 4) and the second-order terms DA2_l are stored as one bf16 plane
   float* c_sdf = nullptr;
   float* HP = nullptr;
@@ -75,7 +72,7 @@ struct nrw_ctx {
   // backward
   nrw::Planes DQ0, DQodd, DQeven, DQ4, DA[2], DFEAT;
   float* DQ8f = nullptr;
-  float* DA2[8] = {nullptr};
+  nrw::SideStream DA2[8];    // second-order terms of the tangent sweep; one bf16 plane when aux_bf16
   nrw::Planes dX[2], dH2, dH1, dXF, dNA[2], dNF, dNH[2];
   float *tail = nullptr, *c_dn = nullptr, *c_ddens = nullptr, *c_dpre3 = nullptr;
   float* gs = nullptr;       // gradient scratch (packed layout)

@@ -2,8 +2,8 @@
 //
 // For an accumulator element acc(m,n) of D = A * B^T the epilogue computes, in this order,
 //   v  = acc [+ bias[n]] [+ rowvec[m]*colvec[n]]
-//   out_pre[m,n] = v                                   (optional fp32 store, all N columns)
-//   w  = gate ? v * softplus100'(a[m,n]) : act(v)        gate: aux_sig (fp32 a) or aux_u (planes of softplus100(a))
+//   out_pre[m,n] = v                                   (optional store, all N columns)
+//   w  = gate ? v * softplus100'(a[m,n]) : act(v)        gate: aux_u (planes of u = softplus100(a))
 //   out2[m,n] = scale * v * aux_q[m,n] * softplus100''(a[m,n])   (optional)
 //   w  = aux_relu ? (aux_relu[m,n] > 0 ? w : 0) : w
 //   w  = w * scale [+ aux_add[m,n]]
@@ -19,35 +19,42 @@ namespace nrw {
 
 enum { ACT_NONE = 0, ACT_SOFTPLUS100 = 1, ACT_RELU = 2, ACT_SIGMOID = 3 };
 
+// Element type of a side stream: fp32, or one rounded bf16 plane (the backward-only streams of the `mixed` mode)
+enum SideType : int { SIDE_F32 = 0, SIDE_BF16 = 1 };
+
+// An optional [rows][ld] side stream of the epilogue (absent: p == nullptr).
+struct SideStream {
+  void* p = nullptr;
+  int ld = 0;
+  SideType type = SIDE_F32;
+  __host__ __device__ explicit operator bool() const { return p != nullptr; }
+  __host__ __device__ float* f32() const { return static_cast<float*>(p); }
+  __host__ __device__ bf16* h() const { return static_cast<bf16*>(p); }
+  __host__ __device__ bool is_bf16() const { return type == SIDE_BF16; }
+  int elem_bytes() const { return p ? (type == SIDE_BF16 ? 2 : 4) : 0; }   // 0 when absent
+};
+inline SideStream side_f32(const float* p, int ld) { return SideStream{const_cast<float*>(p), ld, SIDE_F32}; }
+inline SideStream side_bf16(const bf16* p, int ld) { return SideStream{const_cast<bf16*>(p), ld, SIDE_BF16}; }
+
 struct Epi {
   const float* bias = nullptr;
   const float* rowvec = nullptr;
   const float* colvec = nullptr;
-  const float* aux_sig = nullptr;   // fp32 pre-activation a (legacy / test hook) ...
-  Planes aux_u = {nullptr, 0, 0};   // ... or the bf16 planes of u = softplus100(a) / aux_u_scale that the forward pass kept
+  Planes aux_u = {nullptr, 0, 0};   // the bf16 planes of u = softplus100(a) / aux_u_scale that the forward pass kept
   int aux_u_planes = 0;             //     (planes to read: forward plane count, or 1 for a cheaper backward gate)
   float aux_u_scale = 1.0f;         //     u = aux_u_scale * sum(planes)   (sqrt(2) for the skip layer's input)
-  const float* aux_q = nullptr;
-  const float* aux_add = nullptr;
+  SideStream aux_q;
   int aux_q_bcast = 0;  // aux_q is a [N] row vector broadcast over rows
-  int ld_aux = 0;       // shared by aux_sig / aux_q / aux_add
+  SideStream aux_add;
   const bf16* aux_relu = nullptr;
   int ld_relu = 0;
   int act = ACT_NONE;
   float scale = 1.0f;
-  float* out_pre = nullptr;
-  int ld_pre = 0;
-  // bf16 (single rounded plane) variants of three fp32 side streams that only the BACKWARD pass of the `mixed` mode
-  // consumes - same leading dimensions as their fp32 twins (ld_pre / ld_aux / ld_out2), at most one of each pair is set:
-  bf16* out_pre_h = nullptr;        // Q_l of the gradient chain (read back as aux_q_h by the tangent sweep)
-  const bf16* aux_q_h = nullptr;
-  bf16* out2_h = nullptr;           // second-order term of the tangent sweep (read back as aux_add_h by the reverse sweep)
-  const bf16* aux_add_h = nullptr;
+  SideStream out_pre;   // mixed: Q_l of the gradient chain in bf16 (read back as aux_q by the tangent sweep)
   float* out_f32 = nullptr;
   int ld_f32 = 0;
   int atomic = 0;
-  float* out2 = nullptr;
-  int ld_out2 = 0;
+  SideStream out2;      // mixed: second-order term of the tangent sweep in bf16 (read back as aux_add by the reverse sweep)
   Planes out_pl = {nullptr, 0, 0};
   int n_planes = 0;
   int n_store = 1 << 30;  // column bound for out_f32 / out_pl / out2
@@ -136,18 +143,16 @@ __device__ __forceinline__ void epi_bias(const Epi& e, int m, int n0, int n_all,
   }
 }
 
-// pure register math.  a = aux_sig row, q = aux_q row (in: q, out: out2 values), ad = aux_add row,
-// pos = bit j set <=> forward activation j was > 0.  Returns w (main output).
+// pure register math.  a = u row (softplus100 of the pre-activation), q = aux_q row (in: q, out: out2 values),
+// ad = aux_add row, pos = bit j set <=> forward activation j was > 0.  Returns w (main output).
 template <int NC>
 __device__ __forceinline__ void epi_math(const Epi& e, const float (&acc)[NC], const float (&a)[NC], float (&q)[NC],
                                          const float (&ad)[NC], uint32_t pos, float (&w)[NC]) {
-  if (e.aux_sig || e.aux_u.p) {
-    const bool from_u = e.aux_u.p != nullptr;      // a[] holds u = softplus100(pre-activation) instead of the pre-activation
+  if (e.aux_u.p) {
 #pragma unroll
     for (int j = 0; j < NC; ++j) {
       float s1, s2;
-      if (from_u) softplus100_d12_from_u(a[j], s1, s2);
-      else softplus100_d12(a[j], s1, s2);
+      softplus100_d12_from_u(a[j], s1, s2);
       w[j] = acc[j] * s1 * e.scale;
       if (e.out2) q[j] = e.scale * acc[j] * q[j] * s2;
     }
@@ -187,7 +192,7 @@ __device__ __forceinline__ void epi_apply(const Epi& e, int m, int n0, float (&a
   const int n_all = min(N - n0, NC);
   const int n_st = min(e.n_store - n0, n_all);
   epi_bias<NC>(e, m, n0, n_all, acc);
-  if (e.out_pre) store_f32<NC>(e.out_pre + (long long)m * e.ld_pre + n0, n_all, acc);
+  if (e.out_pre) store_f32<NC>(e.out_pre.f32() + (long long)m * e.out_pre.ld + n0, n_all, acc);
   if (n_st <= 0) return;
   if (e.atomic) {
     float* dst = e.out_f32 + (long long)m * e.ld_f32 + n0;
@@ -200,17 +205,16 @@ __device__ __forceinline__ void epi_apply(const Epi& e, int m, int n0, float (&a
   uint32_t pos = 0;
 #pragma unroll
   for (int j = 0; j < NC; ++j) a[j] = q[j] = ad[j] = 0.0f;
-  if (e.aux_sig) load_f32<NC>(e.aux_sig + (long long)m * e.ld_aux + n0, n_st, a);
   if (e.aux_u.p) {
 #pragma unroll
     for (int j = 0; j < NC; ++j)
       if (j < n_st) a[j] = e.aux_u_scale * planes_load(e.aux_u, e.aux_u_planes, (long long)m * e.aux_u.ld + n0 + j);
   }
   if (e.out2) {
-    if (e.aux_q_bcast) load_f32<NC>(e.aux_q + n0, n_st, q);
-    else load_f32<NC>(e.aux_q + (long long)m * e.ld_aux + n0, n_st, q);
+    if (e.aux_q_bcast) load_f32<NC>(e.aux_q.f32() + n0, n_st, q);
+    else load_f32<NC>(e.aux_q.f32() + (long long)m * e.aux_q.ld + n0, n_st, q);
   }
-  if (e.aux_add) load_f32<NC>(e.aux_add + (long long)m * e.ld_aux + n0, n_st, ad);
+  if (e.aux_add) load_f32<NC>(e.aux_add.f32() + (long long)m * e.aux_add.ld + n0, n_st, ad);
   if (e.aux_relu) {
 #pragma unroll
     for (int j = 0; j < NC; ++j)
@@ -222,7 +226,7 @@ __device__ __forceinline__ void epi_apply(const Epi& e, int m, int n0, float (&a
     for (int j = 0; j < NC; ++j)
       if (j < n_st) atomicAdd(e.colsum + n0 + j, w[j]);
   }
-  if (e.out2) store_f32<NC>(e.out2 + (long long)m * e.ld_out2 + n0, n_st, q);
+  if (e.out2) store_f32<NC>(e.out2.f32() + (long long)m * e.out2.ld + n0, n_st, q);
   if (e.out_f32) store_f32<NC>(e.out_f32 + (long long)m * e.ld_f32 + n0, n_st, w);
   if (e.n_planes > 0) store_planes<NC>(e.out_pl, e.n_planes, (long long)m * e.out_pl.ld + n0, n_st, w);
 }

@@ -7,6 +7,10 @@
 // every auxiliary load and every store of the epilogue is a direct, sector-aligned global access (8 rows
 // x 64 B per fp32 instruction, 8 rows x 32 B per bf16 instruction) and all arithmetic is elementwise, so
 // nothing else goes through shared memory.
+//
+// This file is the line-layout I/O layer both chunk epilogues use (the generic epi_chunk16 below and the specialised kinds of
+// epilogue_fast.cuh): the transpose, the full-tile accessors, the line accessors with their ragged / unaligned fallbacks, bf16
+// packing and column sums.
 #pragma once
 #include "epilogue.cuh"
 
@@ -22,15 +26,96 @@ struct LineLayout {
 __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 __device__ __forceinline__ bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
 
-// tile origin `src` = &matrix[m0w][nc]
+// The one transpose: v = row `lane` of the chunk -> x[4*it + k] = row it*8 + (lane>>2), column 4*(lane&3) + k.
+// stg: this warp's 2 KB tile (64-byte rows, slot' = slot ^ ((row >> 1) & 3)); it may be overwritten again on return.
+__device__ __forceinline__ void line_transpose(float* stg, const float (&v)[16], int lane, float (&x)[16]) {
+  const int sl = lane & 3, r0 = lane >> 2;
+#pragma unroll
+  for (int s = 0; s < 4; ++s)
+    *reinterpret_cast<float4*>(stg + lane * 16 + ((s ^ ((lane >> 1) & 3)) << 2)) = make_float4(v[4 * s], v[4 * s + 1], v[4 * s + 2], v[4 * s + 3]);
+  __syncwarp();
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const int rr = it * 8 + r0;
+    const float4 t = *reinterpret_cast<const float4*>(stg + rr * 16 + ((sl ^ ((rr >> 1) & 3)) << 2));
+    x[4 * it] = t.x; x[4 * it + 1] = t.y; x[4 * it + 2] = t.z; x[4 * it + 3] = t.w;
+  }
+  __syncwarp();
+}
+
+// Side-stream loads.  Warps working on neighbouring column chunks of the same rows read NEIGHBOURING 64-byte (fp32) /
+// 32-byte (bf16) pieces of the same rows, so the first of them asks L2 to fetch the whole aligned 256 bytes
+// (ld.global.nc.L2::256B): the other three find their sectors in L2 instead of queueing a second HBM round trip.
+__device__ __forceinline__ float4 ldg4(const float* p) {
+  float4 v;
+  asm volatile("ld.global.nc.L2::256B.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ uint2 ldg2u(const bf16* p) {
+  uint2 v;
+  asm volatile("ld.global.nc.L2::256B.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p));
+  return v;
+}
+
+// ---- full-tile accessors: all 32 rows and 16 columns valid, 16-byte aligned rows.  p = this lane's first element (row r0,
+// column 4*sl of the tile); o[4*it + k] = p[it*8*ld + k]. ----
+__device__ __forceinline__ void tile_load_f32(const float* p, long long ld, float (&o)[16]) {
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const float4 t = ldg4(p + it * 8 * ld);
+    o[4 * it] = t.x; o[4 * it + 1] = t.y; o[4 * it + 2] = t.z; o[4 * it + 3] = t.w;
+  }
+}
+__device__ __forceinline__ void tile_load_bf16(const bf16* p, long long ld, float (&o)[16]) {
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const uint2 t = ldg2u(p + it * 8 * ld);
+    o[4 * it] = __uint_as_float(t.x << 16); o[4 * it + 1] = __uint_as_float(t.x & 0xFFFF0000u);
+    o[4 * it + 2] = __uint_as_float(t.y << 16); o[4 * it + 3] = __uint_as_float(t.y & 0xFFFF0000u);
+  }
+}
+__device__ __forceinline__ void tile_store_f32(float* p, long long ld, const float (&o)[16]) {
+#pragma unroll
+  for (int it = 0; it < 4; ++it)
+    *reinterpret_cast<float4*>(p + it * 8 * ld) = make_float4(o[4 * it], o[4 * it + 1], o[4 * it + 2], o[4 * it + 3]);
+}
+// pk[2*it], pk[2*it+1] = the 4 bf16 of row it*8+r0
+__device__ __forceinline__ void tile_store_bf16(bf16* p, long long ld, const uint32_t (&pk)[8]) {
+#pragma unroll
+  for (int it = 0; it < 4; ++it) *reinterpret_cast<uint2*>(p + it * 8 * ld) = make_uint2(pk[2 * it], pk[2 * it + 1]);
+}
+// w rounded to bf16 pairs without keeping the residual (split_plane<16> keeps it)
+__device__ __forceinline__ void pack_bf16(const float (&w)[16], uint32_t (&pk)[8]) {
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(w[2 * t], w[2 * t + 1]);
+    pk[t] = *reinterpret_cast<const uint32_t*>(&h);
+  }
+}
+// a side stream's full tile at this lane's first element (row, col)
+__device__ __forceinline__ void tile_load(const SideStream& s, long long row, int col, float (&o)[16]) {
+  if (s.is_bf16()) tile_load_bf16(s.h() + row * s.ld + col, s.ld, o);
+  else tile_load_f32(s.f32() + row * s.ld + col, s.ld, o);
+}
+__device__ __forceinline__ void tile_store(const SideStream& s, long long row, int col, const float (&o)[16]) {
+  if (s.is_bf16()) {
+    uint32_t pk[8];
+    pack_bf16(o, pk);
+    tile_store_bf16(s.h() + row * s.ld + col, s.ld, pk);
+  } else {
+    tile_store_f32(s.f32() + row * s.ld + col, s.ld, o);
+  }
+}
+
+// ---- line accessors of the generic epilogue: any chunk (rows < L.rows_valid, columns < ncols), any alignment; full aligned
+// tiles take the full-tile accessors.  `src` / `dst` = tile origin &matrix[m0w][nc]. ----
+__device__ __forceinline__ bool line_fast(const LineLayout& L, const void* p, long long ld, int ncols) {
+  return L.full && ncols >= 16 && aligned16(p) && (ld & 3) == 0;
+}
 __device__ __forceinline__ void line_load_f32(const LineLayout& L, const float* __restrict__ src, long long ld, int ncols,
                                               float (&o)[16]) {
-  if (L.full && ncols >= 16 && aligned16(src) && (ld & 3) == 0) {
-#pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const float4 t = __ldg(reinterpret_cast<const float4*>(src + (long long)(it * 8 + L.r0) * ld + L.sl * 4));
-      o[4 * it] = t.x; o[4 * it + 1] = t.y; o[4 * it + 2] = t.z; o[4 * it + 3] = t.w;
-    }
+  if (line_fast(L, src, ld, ncols)) {
+    tile_load_f32(src + L.r0 * ld + L.sl * 4, ld, o);
     return;
   }
 #pragma unroll
@@ -45,11 +130,8 @@ __device__ __forceinline__ void line_load_f32(const LineLayout& L, const float* 
 }
 __device__ __forceinline__ void line_store_f32(const LineLayout& L, float* __restrict__ dst, long long ld, int ncols,
                                                const float (&o)[16], bool atomic) {
-  if (!atomic && L.full && ncols >= 16 && aligned16(dst) && (ld & 3) == 0) {
-#pragma unroll
-    for (int it = 0; it < 4; ++it)
-      *reinterpret_cast<float4*>(dst + (long long)(it * 8 + L.r0) * ld + L.sl * 4) =
-          make_float4(o[4 * it], o[4 * it + 1], o[4 * it + 2], o[4 * it + 3]);
+  if (!atomic && line_fast(L, dst, ld, ncols)) {
+    tile_store_f32(dst + L.r0 * ld + L.sl * 4, ld, o);
     return;
   }
 #pragma unroll
@@ -65,13 +147,10 @@ __device__ __forceinline__ void line_store_f32(const LineLayout& L, float* __res
     }
   }
 }
-// pk[2*it], pk[2*it+1] = the 4 bf16 of row it*8+r0
 __device__ __forceinline__ void line_store_bf16(const LineLayout& L, bf16* __restrict__ dst, long long ld, int ncols,
                                                 const uint32_t (&pk)[8]) {
   if (L.full && ncols >= 16 && aligned8(dst) && (ld & 3) == 0) {
-#pragma unroll
-    for (int it = 0; it < 4; ++it)
-      *reinterpret_cast<uint2*>(dst + (long long)(it * 8 + L.r0) * ld + L.sl * 4) = make_uint2(pk[2 * it], pk[2 * it + 1]);
+    tile_store_bf16(dst + L.r0 * ld + L.sl * 4, ld, pk);
     return;
   }
 #pragma unroll
@@ -93,14 +172,10 @@ __device__ __forceinline__ void line_load_planes(const LineLayout& L, const Plan
   for (int pl = 0; pl < n_planes; ++pl) {
     const bf16* src = P.plane(pl) + m0w * P.ld + nc;
     if (L.full && ncols >= 16 && aligned8(src) && (P.ld & 3) == 0) {
+      float t[16];
+      tile_load_bf16(src + L.r0 * P.ld + L.sl * 4, P.ld, t);
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const uint2 t = __ldg(reinterpret_cast<const uint2*>(src + (long long)(it * 8 + L.r0) * P.ld + L.sl * 4));
-        o[4 * it] += __uint_as_float(t.x << 16);
-        o[4 * it + 1] += __uint_as_float(t.x & 0xFFFF0000u);
-        o[4 * it + 2] += __uint_as_float(t.y << 16);
-        o[4 * it + 3] += __uint_as_float(t.y & 0xFFFF0000u);
-      }
+      for (int i = 0; i < 16; ++i) o[i] += t[i];
     } else {
 #pragma unroll
       for (int it = 0; it < 4; ++it) {
@@ -118,34 +193,6 @@ __device__ __forceinline__ void line_load_planes(const LineLayout& L, const Plan
     for (int i = 0; i < 16; ++i) o[i] *= scale;
   }
 }
-// bit e (= 4*it + k) set <=> src[row it*8+r0][col 4*sl+k] > 0
-__device__ __forceinline__ uint32_t line_load_posmask(const LineLayout& L, const bf16* __restrict__ src, long long ld, int ncols) {
-  uint32_t pos = 0;
-  if (L.full && ncols >= 16 && aligned8(src) && (ld & 3) == 0) {
-#pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const uint2 t = __ldg(reinterpret_cast<const uint2*>(src + (long long)(it * 8 + L.r0) * ld + L.sl * 4));
-      const uint32_t u[2] = {t.x, t.y};
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint32_t lo = u[h] & 0xFFFFu, hi = u[h] >> 16;
-        if (lo != 0u && lo < 0x8000u) pos |= 1u << (4 * it + 2 * h);
-        if (hi != 0u && hi < 0x8000u) pos |= 1u << (4 * it + 2 * h + 1);
-      }
-    }
-    return pos;
-  }
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int rr = it * 8 + L.r0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int c = L.sl * 4 + k;
-      if (rr < L.rows_valid && c < ncols && __bfloat162float(src[(long long)rr * ld + c]) > 0.0f) pos |= 1u << (4 * it + k);
-    }
-  }
-  return pos;
-}
 // per-column [N] vector: the 4 values of this lane's column slot
 __device__ __forceinline__ void line_load_cols(const LineLayout& L, const float* __restrict__ vec, int ncols, float (&b)[4]) {
   const float* p = vec + L.sl * 4;
@@ -157,9 +204,44 @@ __device__ __forceinline__ void line_load_cols(const LineLayout& L, const float*
     for (int k = 0; k < 4; ++k) b[k] = (L.sl * 4 + k < ncols) ? p[k] : 0.0f;
   }
 }
+__device__ __forceinline__ void line_load(const LineLayout& L, const SideStream& s, long long m0w, int nc, int ncols, float (&o)[16]) {
+  if (s.is_bf16()) line_load_planes(L, Planes{s.h(), 0, s.ld}, 1, m0w, nc, ncols, 1.0f, o);
+  else line_load_f32(L, s.f32() + m0w * s.ld + nc, s.ld, ncols, o);
+}
+__device__ __forceinline__ void line_store(const LineLayout& L, const SideStream& s, long long m0w, int nc, int ncols,
+                                           const float (&o)[16]) {
+  if (s.is_bf16()) {
+    uint32_t pk[8];
+    pack_bf16(o, pk);
+    line_store_bf16(L, s.h() + m0w * s.ld + nc, s.ld, ncols, pk);
+  } else {
+    line_store_f32(L, s.f32() + m0w * s.ld + nc, s.ld, ncols, o, false);
+  }
+}
+
+// column sums of a 32 x 16 line-layout tile into this CTA's shared accumulator cs_tile[16]: rows first (registers), then a
+// halving butterfly over the 8 lanes that share a column slot: 4 SHFL instead of 12
+__device__ __forceinline__ void line_colsum_add(const float (&w)[16], int lane, float* cs_tile) {
+  float c0 = (w[0] + w[4]) + (w[8] + w[12]), c1 = (w[1] + w[5]) + (w[9] + w[13]);
+  float c2 = (w[2] + w[6]) + (w[10] + w[14]), c3 = (w[3] + w[7]) + (w[11] + w[15]);
+  const bool hi16 = (lane & 16) != 0, hi8 = (lane & 8) != 0;
+  // round 1 (xor 16): lanes with bit 4 clear keep columns 0,1; the others keep 2,3
+  const float s0 = hi16 ? c0 : c2, s1 = hi16 ? c1 : c3;
+  float k0 = hi16 ? c2 : c0, k1 = hi16 ? c3 : c1;
+  k0 += __shfl_xor_sync(0xFFFFFFFFu, s0, 16);
+  k1 += __shfl_xor_sync(0xFFFFFFFFu, s1, 16);
+  // round 2 (xor 8): bit 3 clear keeps the first of the two, set keeps the second
+  const float s = hi8 ? k0 : k1;
+  float k = hi8 ? k1 : k0;
+  k += __shfl_xor_sync(0xFFFFFFFFu, s, 8);
+  // round 3 (xor 4): both partners hold the same column
+  k += __shfl_xor_sync(0xFFFFFFFFu, k, 4);
+  if ((lane & 4) == 0) atomicAdd(cs_tile + (lane & 3) * 4 + (hi16 ? 2 : 0) + (hi8 ? 1 : 0), k);   // shared-memory reduction
+}
 
 // v: row `lane` of the accumulator chunk (columns nc..nc+15 of rows m0w..m0w+31).  stg: this warp's 2 KB tile.
-// cs_tile: this CTA's shared column-sum accumulator for columns nc..nc+15 (flushed by the kernel), or nullptr.
+// cs_tile: this CTA's shared column-sum accumulator for columns nc..nc+15 (flushed by the kernel); non-null iff e.colsum is set
+// and the epilogue is not atomic.
 __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const float (&v)[16], int m0w, int nc, int M, int N, int lane,
                                             float* cs_tile) {
   LineLayout L;
@@ -170,19 +252,8 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const floa
   L.sl = lane & 3;
   L.r0 = lane >> 2;
   L.full = L.rows_valid == 32;
-  // ---- the one transpose: row layout -> line layout (64-byte rows, slot' = slot ^ ((row >> 1) & 3)) ----
-#pragma unroll
-  for (int s = 0; s < 4; ++s)
-    *reinterpret_cast<float4*>(stg + lane * 16 + ((s ^ ((lane >> 1) & 3)) << 2)) = make_float4(v[4 * s], v[4 * s + 1], v[4 * s + 2], v[4 * s + 3]);
-  __syncwarp();
   float x[16];
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int rr = it * 8 + L.r0;
-    const float4 t = *reinterpret_cast<const float4*>(stg + rr * 16 + ((L.sl ^ ((rr >> 1) & 3)) << 2));
-    x[4 * it] = t.x; x[4 * it + 1] = t.y; x[4 * it + 2] = t.z; x[4 * it + 3] = t.w;
-  }
-  __syncwarp();   // the tile may be overwritten by the next chunk from here on
+  line_transpose(stg, v, lane, x);
   // ---- v = acc + bias + rowvec * colvec ----
   if (e.bias) {
     float b[4];
@@ -200,16 +271,7 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const floa
       for (int k = 0; k < 4; ++k) x[4 * it + k] = fmaf(rv, cv[k], x[4 * it + k]);
     }
   }
-  if (e.out_pre) line_store_f32(L, e.out_pre + (long long)m0w * e.ld_pre + nc, e.ld_pre, n_all, x, false);
-  if (e.out_pre_h) {
-    uint32_t pk[8];
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-      const __nv_bfloat162 h = __floats2bfloat162_rn(x[2 * t], x[2 * t + 1]);
-      pk[t] = *reinterpret_cast<const uint32_t*>(&h);
-    }
-    line_store_bf16(L, e.out_pre_h + (long long)m0w * e.ld_pre + nc, e.ld_pre, n_all, pk);
-  }
+  if (e.out_pre) line_store(L, e.out_pre, m0w, nc, n_all, x);
   if (n_st <= 0) return;
   if (e.atomic) {
     if (e.scale != 1.0f) {
@@ -221,48 +283,32 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const floa
   }
   // ---- activation / gating (elementwise, see epilogue.cuh) ----
   float w[16];
-  if (e.aux_sig || e.aux_u.p) {
-    float a[16];
-    const bool from_u = e.aux_u.p != nullptr;     // gate from the stored softplus OUTPUT planes (no fp32 pre-activation in HBM)
-    if (from_u) line_load_planes(L, e.aux_u, e.aux_u_planes, m0w, nc, n_st, e.aux_u_scale, a);
-    else line_load_f32(L, e.aux_sig + (long long)m0w * e.ld_aux + nc, e.ld_aux, n_st, a);
-    if (e.out2 || e.out2_h) {
+  if (e.aux_u.p) {
+    float a[16];   // the gate from the stored softplus OUTPUT planes (no fp32 pre-activation in HBM)
+    line_load_planes(L, e.aux_u, e.aux_u_planes, m0w, nc, n_st, e.aux_u_scale, a);
+    if (e.out2) {
       float q[16];
-      if (e.aux_q_h) {
-        line_load_planes(L, Planes{const_cast<bf16*>(e.aux_q_h), 0, e.ld_aux}, 1, m0w, nc, n_st, 1.0f, q);
-      } else if (e.aux_q_bcast) {
+      if (e.aux_q_bcast) {
         float qb[4];
-        line_load_cols(L, e.aux_q + nc, n_st, qb);
+        line_load_cols(L, e.aux_q.f32() + nc, n_st, qb);
 #pragma unroll
         for (int i = 0; i < 16; ++i) q[i] = qb[i & 3];
       } else {
-        line_load_f32(L, e.aux_q + (long long)m0w * e.ld_aux + nc, e.ld_aux, n_st, q);
+        line_load(L, e.aux_q, m0w, nc, n_st, q);
       }
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         float s1, s2;
-        if (from_u) softplus100_d12_from_u(a[i], s1, s2);
-        else softplus100_d12(a[i], s1, s2);
+        softplus100_d12_from_u(a[i], s1, s2);
         w[i] = x[i] * s1 * e.scale;
         q[i] = e.scale * x[i] * q[i] * s2;
       }
-      if (e.out2_h) {
-        uint32_t pk[8];
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          const __nv_bfloat162 h = __floats2bfloat162_rn(q[2 * t], q[2 * t + 1]);
-          pk[t] = *reinterpret_cast<const uint32_t*>(&h);
-        }
-        line_store_bf16(L, e.out2_h + (long long)m0w * e.ld_out2 + nc, e.ld_out2, n_st, pk);
-      } else {
-        line_store_f32(L, e.out2 + (long long)m0w * e.ld_out2 + nc, e.ld_out2, n_st, q, false);
-      }
+      line_store(L, e.out2, m0w, nc, n_st, q);
     } else {
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         float s1, s2;
-        if (from_u) softplus100_d12_from_u(a[i], s1, s2);
-        else softplus100_d12(a[i], s1, s2);
+        softplus100_d12_from_u(a[i], s1, s2);
         w[i] = x[i] * s1 * e.scale;
       }
     }
@@ -285,38 +331,25 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const floa
         for (int i = 0; i < 16; ++i) w[i] = x[i] * e.scale;
     }
     if (e.aux_relu) {
-      const uint32_t pos = line_load_posmask(L, e.aux_relu + (long long)m0w * e.ld_relu + nc, e.ld_relu, n_st);
+      float f[16];   // forward activation: 0 outside the chunk
+      line_load_planes(L, Planes{const_cast<bf16*>(e.aux_relu), 0, e.ld_relu}, 1, m0w, nc, n_st, 1.0f, f);
 #pragma unroll
       for (int i = 0; i < 16; ++i)
-        if (!((pos >> i) & 1u)) w[i] = 0.0f;
+        if (!(f[i] > 0.0f)) w[i] = 0.0f;
     }
   }
-  if (e.aux_add || e.aux_add_h) {
+  if (e.aux_add) {
     float ad[16];
-    if (e.aux_add_h) line_load_planes(L, Planes{const_cast<bf16*>(e.aux_add_h), 0, e.ld_aux}, 1, m0w, nc, n_st, 1.0f, ad);
-    else line_load_f32(L, e.aux_add + (long long)m0w * e.ld_aux + nc, e.ld_aux, n_st, ad);
+    line_load(L, e.aux_add, m0w, nc, n_st, ad);
 #pragma unroll
     for (int i = 0; i < 16; ++i) w[i] += ad[i];
   }
-  if (e.colsum) {
-    // column sums over the 32 rows: 4 rows per lane, then the 8 lanes sharing a column slot
-    float cs[4];
+  if (cs_tile) {
+    // rows and columns outside the chunk add nothing: the accumulator's entries at or beyond the tile's column count stay zero
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      cs[k] = 0.0f;
-#pragma unroll
-      for (int it = 0; it < 4; ++it) cs[k] += (it * 8 + L.r0 < L.rows_valid) ? w[4 * it + k] : 0.0f;
-#pragma unroll
-      for (int o = 4; o < 32; o <<= 1) cs[k] += __shfl_xor_sync(0xFFFFFFFFu, cs[k], o);
-    }
-    if (lane < 4) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (lane * 4 + k < n_st) {
-          if (cs_tile) atomicAdd(cs_tile + lane * 4 + k, cs[k]);   // shared-memory reduction (same-address global atomics serialise)
-          else atomicAdd(e.colsum + nc + lane * 4 + k, cs[k]);
-        }
-    }
+    for (int i = 0; i < 16; ++i)
+      if ((i >> 2) * 8 + L.r0 >= L.rows_valid || L.sl * 4 + (i & 3) >= n_st) w[i] = 0.0f;
+    line_colsum_add(w, lane, cs_tile);
   }
   if (e.out_f32) line_store_f32(L, e.out_f32 + (long long)m0w * e.ld_f32 + nc, e.ld_f32, n_st, w, false);
   for (int pl = 0; pl < e.n_planes; ++pl) {
@@ -326,8 +359,8 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const floa
   }
 }
 
-// Column-sum accumulator of one consumer warpgroup (the n_cols columns of its current n-tile; the chunk epilogues never
-// touch an entry beyond n_cols, so those stay zero).  All `n_threads` threads of the warpgroup call this together (named
+// Column-sum accumulator of one consumer warpgroup (the n_cols columns of its current n-tile; the chunk epilogues add only
+// zeros to the entries beyond n_cols, so those stay zero).  All `n_threads` threads of the warpgroup call this together (named
 // barrier `bar_id`): adds the tile's partial sums to global memory and clears the accumulator.
 __device__ __forceinline__ void colsum_flush(float* cs, float* __restrict__ colsum, int n0, int n_cols, int tid, int n_threads,
                                              int bar_id) {

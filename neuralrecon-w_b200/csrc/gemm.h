@@ -14,15 +14,14 @@ struct GemmDesc {
   Epi epi;
 };
 
-enum GemmBackend { GEMM_TCGEN05 = 0, GEMM_SIMT = 1 };
-
 // wgmma / TMA tensor-core implementation (gemm_tc.cu)
 int gemm_tc(const GemmDesc& g, cudaStream_t stream);
 // fp32 CUDA-core implementation over the same operands (gemm_simt.cu); verification backend
 int gemm_simt(const GemmDesc& g, cudaStream_t stream);
 
+// backend: NRW_GEMM_TCGEN05 or NRW_GEMM_SIMT (nrw.h)
 inline int gemm(int backend, const GemmDesc& g, cudaStream_t stream) {
-  return backend == GEMM_SIMT ? gemm_simt(g, stream) : gemm_tc(g, stream);
+  return backend == NRW_GEMM_SIMT ? gemm_simt(g, stream) : gemm_tc(g, stream);
 }
 
 // number of (a_plane, b_plane) products issued for a given plane count: 1, 3, 6

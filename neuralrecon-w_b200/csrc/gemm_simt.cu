@@ -71,7 +71,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(Planes A, Planes B, int 
 int gemm_simt(const GemmDesc& g, cudaStream_t stream) {
   NRW_CHECK(g.M > 0 && g.N > 0 && g.K > 0, NRW_ERR_ARG, "gemm_simt: empty problem");
   NRW_CHECK(g.k_slices == 1 || g.epi.atomic, NRW_ERR_ARG, "gemm_simt: split-K needs an atomic epilogue");
-  NRW_CHECK(!g.epi.out_pre_h && !g.epi.out2_h && !g.epi.aux_q_h && !g.epi.aux_add_h && !g.epi.head_w, NRW_ERR_ARG,
+  NRW_CHECK(!g.epi.out_pre.is_bf16() && !g.epi.out2.is_bf16() && !g.epi.aux_q.is_bf16() && !g.epi.aux_add.is_bf16() && !g.epi.head_w, NRW_ERR_ARG,
             "gemm_simt: bf16 side streams are a tensor-core-path feature");
   dim3 grid(cdiv(g.N, TN), cdiv(g.M, TM), g.k_slices);
   if (g.mn_major)

@@ -408,7 +408,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
           named_bar_sync(2 + wg, 128);               // the staging tile is free: it holds the warps' 2 KB tiles from here on
           const int nc = n0 + 32 * cp + 16 * cc;
           if (nc < p.N && m0w < p.M)                 // warp-uniform
-            epi_fast16<EK>(p.epi, stg, v, m0w, nc, p.M, p.N, lane, use_cs ? cs_wg + 32 * cp + 16 * cc : nullptr, nullptr, 0, hacc);
+            epi_fast16<EK>(p.epi, stg, v, m0w, nc, p.M, p.N, lane, use_cs ? cs_wg + 32 * cp + 16 * cc : nullptr, hacc);
           named_bar_sync(2 + wg, 128);
         }
         if (EK == EK_FWD_HEAD && (lane & 3) == 0) { // partial[row][slot], slot = n-tile * 2 + column class: plain stores
@@ -561,7 +561,7 @@ static cudaEvent_t get_event() {
 int gemm_tc_timing_read(double* ms, double* flops, double* mma_flops, long long* launches, double* bytes) {
   double t = 0, f = 0, mf = 0, by = 0;
   // tuning: NRW_GEMM_TIMING_DUMP=<path> appends one CSV row per launch: M,N,K,planes,mn_major,k_slices,epilogue bits,
-  // algorithmic bytes,ms   (bits: 1 out_pre 2 out_f32 4 out2 8 planes 16 aux_sig 32 aux_q 64 aux_add 128 aux_relu 256 atomic 512 colsum)
+  // algorithmic bytes,ms   (bits: 1 out_pre 2 out_f32 4 out2 8 planes 16 gate (aux_u) 32 aux_q 64 aux_add 128 aux_relu 256 atomic 512 colsum)
   FILE* dump = getenv("NRW_GEMM_TIMING_DUMP") ? fopen(getenv("NRW_GEMM_TIMING_DUMP"), "a") : nullptr;
   for (auto& L : g_timed) {
     NRW_CUDA_OK(cudaEventSynchronize(L.e1));
@@ -586,14 +586,13 @@ int gemm_tc(const GemmDesc& g, cudaStream_t stream) {
   L.mma_flops = L.flops * n_products(g.n_planes);
   L.M = g.M; L.N = g.N; L.K = g.K; L.P = g.n_planes; L.mn = g.mn_major; L.ks = g.k_slices;
   const Epi& e = g.epi;
-  L.epi = ((e.out_pre || e.out_pre_h) ? 1u : 0u) | (e.out_f32 ? 2u : 0u) | ((e.out2 || e.out2_h) ? 4u : 0u) | (e.n_planes ? 8u : 0u) | ((e.aux_sig || e.aux_u.p) ? 16u : 0u) |
-          (((e.aux_q && !e.aux_q_bcast) || e.aux_q_h) ? 32u : 0u) | ((e.aux_add || e.aux_add_h) ? 64u : 0u) | (e.aux_relu ? 128u : 0u) | (e.atomic ? 256u : 0u) |
-          (e.colsum ? 512u : 0u);
+  const int q_bytes = e.aux_q_bcast ? 0 : e.aux_q.elem_bytes();   // a broadcast row vector is no stream
+  L.epi = (e.out_pre ? 1u : 0u) | (e.out_f32 ? 2u : 0u) | (e.out2 ? 4u : 0u) | (e.n_planes ? 8u : 0u) | (e.aux_u.p ? 16u : 0u) |
+          (q_bytes ? 32u : 0u) | (e.aux_add ? 64u : 0u) | (e.aux_relu ? 128u : 0u) | (e.atomic ? 256u : 0u) | (e.colsum ? 512u : 0u);
   const double mn = (double)g.M * (double)std::min(g.N, e.n_store);
-  L.bytes = 2.0 * g.n_planes * ((double)g.M * g.K + (double)g.N * g.K) + (e.out_pre ? 4.0 * g.M * g.N : 0.0) + (e.out_pre_h ? 2.0 * g.M * g.N : 0.0) +
-            mn * (4.0 * ((e.out_f32 ? 1 : 0) + (e.out2 ? 1 : 0) + (e.aux_sig ? 1 : 0) + ((e.aux_q && !e.aux_q_bcast) ? 1 : 0) +
-                         (e.aux_add ? 1 : 0)) + 2.0 * e.n_planes + (e.aux_relu ? 2.0 : 0.0) + (e.aux_u.p ? 2.0 * e.aux_u_planes : 0.0) +
-                  2.0 * ((e.out2_h ? 1 : 0) + (e.aux_q_h ? 1 : 0) + (e.aux_add_h ? 1 : 0)));
+  L.bytes = 2.0 * g.n_planes * ((double)g.M * g.K + (double)g.N * g.K) + (double)e.out_pre.elem_bytes() * g.M * g.N +
+            mn * (4.0 * (e.out_f32 ? 1 : 0) + e.out2.elem_bytes() + q_bytes + e.aux_add.elem_bytes() + 2.0 * e.n_planes +
+                  (e.aux_relu ? 2.0 : 0.0) + (e.aux_u.p ? 2.0 * e.aux_u_planes : 0.0));
   NRW_CUDA_OK(cudaEventRecord(L.e0, stream));
   const int rc = gemm_tc_impl(g, stream);
   NRW_CUDA_OK(cudaEventRecord(L.e1, stream));
@@ -626,8 +625,7 @@ static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
       NRW_TRY(make_map(&p.tmB[pl], g.B.plane(pl), g.N, g.K, g.B.ld, 64, BK));
     }
   }
-  static const int use_fast = getenv("NRW_EPI_FAST") ? atoi(getenv("NRW_EPI_FAST")) : 1;   // 0: generic epilogue everywhere
-  const int ek = (g.mn_major || (!use_fast && !g.epi.head_w)) ? EK_GENERIC : pick_epi_kind(g.epi);
+  const int ek = g.mn_major ? EK_GENERIC : pick_epi_kind(g.epi);
   NRW_CHECK(ek >= 0 && (ek != EK_FWD_HEAD || g.N == 512), NRW_ERR_ARG,
             "gemm_tc: the fused SDF-head epilogue needs N = 512, bias + softplus and no other output");
   if (g.mn_major) return BN == 64 ? launch<64, 1, EK_GENERIC>(p, n_sm, dev, stream) : launch<128, 1, EK_GENERIC>(p, n_sm, dev, stream);

@@ -36,7 +36,6 @@ def test_gemm_forward_form(backend, shape):
 
 @pytest.mark.parametrize("backend", [0, 1])
 @pytest.mark.parametrize("shape", [(5000, 512, 512, 4), (3000, 128, 640, 3), (2048, 256, 192, 1), (1000, 512, 64, 2),
-                                   # 256 x 512 pair tiles of the one-plane split-K path: two column tiles, a ragged second tile, 3 row tiles
                                    (4100, 256, 1024, 3), (3000, 512, 640, 2), (9000, 768, 512, 5)])
 def test_gemm_weight_gradient_form(backend, shape):
     Ks, M, N, ks = shape
@@ -47,25 +46,6 @@ def test_gemm_weight_gradient_form(backend, shape):
     for planes, tol in ((1, 8e-3), (2, 5e-5), (3, 5e-5)):
         D = gemm_test(backend, planes, 1, ks, A, B, None, 0).cpu()
         assert rel_err(D, ref) < tol, (backend, shape, planes)
-
-
-def test_gemm_weight_gradient_wide_tiles_two_planes():
-    """NRW_DW_WIDE=2 routes two-plane operands through the 256 x 512 tiles as well (2 TMA stages); the switch is read once per
-    process, hence the subprocess."""
-    import subprocess
-    import sys
-    code = (
-        "import sys, numpy as np, torch; sys.path.insert(0, 'tests'); from util_nrw import gemm_test, rel_err\n"
-        "for (Ks, M, N, ks) in ((5000, 512, 512, 4), (3000, 512, 640, 2), (4100, 256, 1024, 3)):\n"
-        "    torch.manual_seed(1); A = torch.randn(Ks, M, device='cuda'); B = torch.randn(Ks, N, device='cuda') / np.sqrt(Ks)\n"
-        "    ref = (A.double().T @ B.double()).float().cpu()\n"
-        "    for planes, tol in ((1, 8e-3), (2, 5e-5)):\n"
-        "        e = rel_err(gemm_test(0, planes, 1, ks, A, B, None, 0).cpu(), ref); assert e < tol, (Ks, M, N, planes, e)\n"
-        "print('wide ok')\n")
-    from conftest import ROOT
-    env = dict(os.environ, NRW_DW_WIDE="2")
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=env, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "wide ok" in r.stdout, r.stdout + r.stderr
 
 
 def test_gemm_epilogue_activations():

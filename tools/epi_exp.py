@@ -1,5 +1,5 @@
-"""Tuning experiment: time ONE 2-CTA GEMM launch (live CUDA events inside the library) for a forward-layer shaped problem.
-Env: NRW_TC_DBG (bit0 drain-only epilogue, bit1 one MMA per k-block), NRW_GEMM_TEST_LAYER=1 (layer store pattern)."""
+"""Tuning experiment: time ONE GEMM launch (live CUDA events inside the library) for a forward-layer shaped problem.
+Env: NRW_GEMM_TEST_LAYER=1 (layer store pattern)."""
 import ctypes as C, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "neuralrecon-w_b200"))
@@ -21,4 +21,4 @@ torch.cuda.synchronize()
 out = (C.c_double * 5)()
 L.nrw_gemm_timing(0, out)
 ms = out[0] / out[3]
-print(f"DBG={os.environ.get('NRW_TC_DBG','0')} LAYER={os.environ.get('NRW_GEMM_TEST_LAYER','0')} M={M} N={N} K={K} P={planes} act={act}: {ms*1e3:.1f} us/launch  mma {out[2]/out[0]/1e9:.0f} TF/s")
+print(f"LAYER={os.environ.get('NRW_GEMM_TEST_LAYER','0')} M={M} N={N} K={K} P={planes} act={act}: {ms*1e3:.1f} us/launch  mma {out[2]/out[0]/1e9:.0f} TF/s")

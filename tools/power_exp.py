@@ -1,5 +1,5 @@
-"""Is the 2-CTA GEMM power-capped?  Runs ~1.5 s of back-to-back launches per NRW_TC_DBG mode (set per process) and
-samples SM clock and board power through NVML meanwhile."""
+"""Is the GEMM power-capped?  Runs ~1.5 s of back-to-back launches of one shape and samples SM clock and board power
+through NVML meanwhile."""
 import ctypes as C, os, sys, threading, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "neuralrecon-w_b200"))
@@ -29,5 +29,5 @@ while time.time() - t0 < 1.5:
 out = (C.c_double * 5)(); L.nrw_gemm_timing(0, out)
 stop.set(); th.join()
 clk.sort(); pw.sort()
-print(f"DBG={os.environ.get('NRW_TC_DBG','0')} LAYER={os.environ.get('NRW_GEMM_TEST_LAYER','0')} P={planes}: {out[0]/out[3]*1e3:.1f} us/launch over {int(out[3])} launches; "
+print(f"LAYER={os.environ.get('NRW_GEMM_TEST_LAYER','0')} P={planes}: {out[0]/out[3]*1e3:.1f} us/launch over {int(out[3])} launches; "
       f"SM clock median {clk[len(clk)//2]} MHz (min {clk[0]}), power median {pw[len(pw)//2]:.0f} W (max {pw[-1]:.0f}), limit {nv.nvmlDeviceGetEnforcedPowerLimit(h)/1e3:.0f} W")
