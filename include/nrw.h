@@ -276,6 +276,28 @@ NRW_API int nrw_mc_count(const float* vol, int d0, int d1, int d2, float level, 
 NRW_API int nrw_mc_emit(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask, const void* scratch,
                         long long n_verts, long long n_faces, float* verts, float* normals, int32_t* faces, void* stream);
 
+/* ---- exact nearest neighbour and surface sampling in fp64 (utils/eval_utils.py; rules in csrc/nnsearch.cu) ----------
+ * nrw_nn_build indexes ref f64 [n_ref,3] (1 <= n_ref <= INT32_MAX, finite) into `index` (nrw_nn_index_bytes(n_ref) bytes,
+ * 256-byte aligned; it also serves as the build's scratch).  nrw_nn_query writes, for every query q of queries f64
+ * [n_query,3], the smallest (squared distance, index) pair over the indexed points: dist f64 [n_query] = sqrt of the
+ * squared distance, idx int64 [n_query].  n_ref must be the count the index was built for (the index holds its own copy of
+ * the points, so `ref` may be freed after the build).  scratch:
+ * nrw_nn_query_scratch_bytes(n_query), 256-byte aligned.  The *_bytes functions return a negative nrw_status for a size
+ * outside their range. */
+NRW_API long long nrw_nn_index_bytes(long long n_ref);
+NRW_API int nrw_nn_build(const double* ref, long long n_ref, void* index, void* stream);
+NRW_API long long nrw_nn_query_scratch_bytes(long long n_query);
+NRW_API int nrw_nn_query(const void* index, long long n_ref, const double* queries, long long n_query, double* dist,
+                         int64_t* idx, void* scratch, void* stream);
+/* Area-weighted uniform samples of the triangle mesh verts f64 [n_verts,3], faces int64 [n_faces,3]: out f64
+ * [n_samples,3], face_id int64 [n_samples] (nullable).  Sample s depends only on (seed, s).  status (device int32[1]) is
+ * written by the call: bit 0 = a face index outside [0, n_verts), bit 1 = total area not positive and finite; when it is
+ * non-zero nothing is sampled.  scratch: nrw_mesh_sample_scratch_bytes(n_faces), 256-byte aligned. */
+NRW_API long long nrw_mesh_sample_scratch_bytes(long long n_faces);
+NRW_API int nrw_mesh_sample(const double* verts, long long n_verts, const int64_t* faces, long long n_faces, long long n_samples,
+                            unsigned long long seed, double* out, int64_t* face_id /*nullable*/, int32_t* status,
+                            void* scratch, void* stream);
+
 /* ---- unit-test hooks ---------------------------------------------------------------------- */
 /* D[M,N] = (sum planes of A)[M,K] * (sum planes of B)[N,K]^T from fp32 inputs: splits into planes in
  * scratch (caller-provided, nrw_gemm_test_scratch_bytes) and runs the selected backend. */

@@ -339,6 +339,27 @@ int nrw_mc_emit(const float* vol, int d0, int d1, int d2, float level, const uin
   NRW_GUARD_END
 }
 
+long long nrw_nn_index_bytes(long long n_ref) { return nn_index_bytes(n_ref); }
+int nrw_nn_build(const double* ref, long long n_ref, void* index, void* stream) {
+  NRW_GUARD_BEGIN
+  return nn_build(ref, n_ref, index, S(stream));
+  NRW_GUARD_END
+}
+long long nrw_nn_query_scratch_bytes(long long n_query) { return nn_query_scratch_bytes(n_query); }
+int nrw_nn_query(const void* index, long long n_ref, const double* queries, long long n_query, double* dist, int64_t* idx,
+                 void* scratch, void* stream) {
+  NRW_GUARD_BEGIN
+  return nn_query(index, n_ref, queries, n_query, dist, idx, scratch, S(stream));
+  NRW_GUARD_END
+}
+long long nrw_mesh_sample_scratch_bytes(long long n_faces) { return mesh_sample_scratch_bytes(n_faces); }
+int nrw_mesh_sample(const double* verts, long long n_verts, const int64_t* faces, long long n_faces, long long n_samples,
+                    unsigned long long seed, double* out, int64_t* face_id, int32_t* status, void* scratch, void* stream) {
+  NRW_GUARD_BEGIN
+  return mesh_sample(verts, n_verts, faces, n_faces, n_samples, seed, out, face_id, status, scratch, S(stream));
+  NRW_GUARD_END
+}
+
 long long nrw_gemm_test_scratch_bytes(int M, int N, int K) {
   const long long a = round_up((long long)M * K, 512), b = round_up((long long)N * K, 512);
   return (a + b) * 3 * 2 + 4096;

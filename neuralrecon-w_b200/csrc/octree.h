@@ -49,3 +49,15 @@ int mc_count(const float* vol, int d0, int d1, int d2, float level, const uint8_
 int mc_emit(const float* vol, int d0, int d1, int d2, float level, const uint8_t* mask, const void* scratch, long long n_verts,
             long long n_faces, float* verts, float* normals, int32_t* faces, cudaStream_t s);
 }  // namespace nrw
+
+// exact fp64 nearest neighbour and area-weighted surface sampling (nnsearch.cu)
+namespace nrw {
+long long nn_index_bytes(long long n_ref);
+int nn_build(const double* ref, long long n_ref, void* index, cudaStream_t s);
+long long nn_query_scratch_bytes(long long n_query);
+int nn_query(const void* index, long long n_ref, const double* queries, long long n_query, double* dist, int64_t* idx,
+             void* scratch, cudaStream_t s);
+long long mesh_sample_scratch_bytes(long long n_faces);
+int mesh_sample(const double* verts, long long n_verts, const int64_t* faces, long long n_faces, long long n_samples,
+                unsigned long long seed, double* out, int64_t* face_id, int32_t* status, void* scratch, cudaStream_t s);
+}  // namespace nrw

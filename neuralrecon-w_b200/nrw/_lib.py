@@ -105,6 +105,15 @@ def lib():
     L.nrw_mc_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_mc_count.argtypes = [vp, i32, i32, i32, f32, vp, vp, vp, vp]
     L.nrw_mc_emit.argtypes = [vp, i32, i32, i32, f32, vp, vp, ll, ll, vp, vp, vp, vp]
+    L.nrw_nn_index_bytes.restype = ll
+    L.nrw_nn_index_bytes.argtypes = [ll]
+    L.nrw_nn_build.argtypes = [vp, ll, vp, vp]
+    L.nrw_nn_query_scratch_bytes.restype = ll
+    L.nrw_nn_query_scratch_bytes.argtypes = [ll]
+    L.nrw_nn_query.argtypes = [vp, ll, vp, ll, vp, vp, vp, vp]
+    L.nrw_mesh_sample_scratch_bytes.restype = ll
+    L.nrw_mesh_sample_scratch_bytes.argtypes = [ll]
+    L.nrw_mesh_sample.argtypes = [vp, ll, vp, ll, ll, C.c_ulonglong, vp, vp, vp, vp, vp]
     L.nrw_gemm_test_scratch_bytes.restype = ll
     L.nrw_gemm_test_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_gemm_test.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp]
@@ -124,7 +133,9 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_gemm_timing", "nrw_ctx_set_backward_planes", "nrw_octree_build_scratch_bytes", "nrw_octree_build",
            "nrw_grad_sumsq", "nrw_adam_clip_step", "nrw_boundary_samples", "nrw_compact_scratch_bytes", "nrw_raycache_gather",
            "nrw_grid_points_dense", "nrw_grid_points_sparse", "nrw_threshold_compact", "nrw_ctx_set_backward_gate_planes",
-           "nrw_mc_scratch_bytes", "nrw_mc_count", "nrw_mc_emit"]
+           "nrw_mc_scratch_bytes", "nrw_mc_count", "nrw_mc_emit",
+           "nrw_nn_index_bytes", "nrw_nn_build", "nrw_nn_query_scratch_bytes", "nrw_nn_query", "nrw_mesh_sample_scratch_bytes",
+           "nrw_mesh_sample"]
 
 
 def check(status, what=""):

@@ -228,49 +228,144 @@ class Mesh:
         write_ply(path, self.vertices, self.faces, self.vertex_normals, self.vertex_colors)
 
 
-def write_ply(path, vertices, faces, normals, colors=None):
-    n, f = len(vertices), len(faces)
-    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+def write_ply(path, vertices, faces=None, normals=None, colors=None):
+    """Binary little-endian PLY: vertex x y z [nx ny nz] (float32) [red green blue (uchar)], and with `faces` a face list
+    uchar int.  faces=None and normals=None write a point cloud."""
+    n = len(vertices)
+    names = ["x", "y", "z"] + (["nx", "ny", "nz"] if normals is not None else [])
+    fields = [(name, "<f4") for name in names]
     if colors is not None:
         fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
     v = np.empty(n, dtype=fields)
     for c, name in enumerate("xyz"):
         v[name] = vertices[:, c]
-        v["n" + name] = normals[:, c]
+        if normals is not None:
+            v["n" + name] = normals[:, c]
     if colors is not None:
         for c, name in enumerate(("red", "green", "blue")):
             v[name] = colors[:, c]
-    fc = np.empty(f, dtype=[("n", "u1"), ("i", "<i4", (3,))])
-    fc["n"] = 3
-    fc["i"] = faces
     head = ["ply", "format binary_little_endian 1.0", f"element vertex {n}"]
-    head += [f"property float {name}" for name in ("x", "y", "z", "nx", "ny", "nz")]
+    head += [f"property float {name}" for name in names]
     if colors is not None:
         head += [f"property uchar {name}" for name in ("red", "green", "blue")]
-    head += [f"element face {f}", "property list uchar int vertex_indices", "end_header"]
+    if faces is not None:
+        fc = np.empty(len(faces), dtype=[("n", "u1"), ("i", "<i4", (3,))])
+        fc["n"] = 3
+        fc["i"] = faces
+        head += [f"element face {len(faces)}", "property list uchar int vertex_indices"]
+    head += ["end_header"]
     with open(path, "wb") as fh:
         fh.write(("\n".join(head) + "\n").encode("ascii"))
         fh.write(v.tobytes())
-        fh.write(fc.tobytes())
+        if faces is not None:
+            fh.write(fc.tobytes())
+
+
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",
+              "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4",
+              "double": "f8", "float64": "f8"}
+
+
+def _ply_header(data):
+    """-> (format, [(element name, count, [(property name, type) or (name, ("list", count type, item type))])], body offset)"""
+    if not data.startswith(b"ply"):
+        raise NrwError("read_ply: not a PLY file")
+    end = data.find(b"end_header")
+    if end < 0:
+        raise NrwError("read_ply: no end_header")
+    body = data.index(b"\n", end) + 1
+    fmt, elems = None, []
+    for line in data[:end].decode("ascii", "replace").splitlines():
+        t = line.split()
+        if not t or t[0] in ("ply", "comment", "obj_info"):
+            continue
+        if t[0] == "format":
+            fmt = t[1]
+        elif t[0] == "element":
+            elems.append((t[1], int(t[2]), []))
+        elif t[0] == "property" and elems:
+            try:
+                if t[1] == "list":
+                    elems[-1][2].append((t[4], ("list", _PLY_TYPES[t[2]], _PLY_TYPES[t[3]])))
+                else:
+                    elems[-1][2].append((t[2], _PLY_TYPES[t[1]]))
+            except KeyError as e:
+                raise NrwError(f"read_ply: unknown property type in {line!r}") from e
+    if fmt not in ("ascii", "binary_little_endian", "binary_big_endian"):
+        raise NrwError(f"read_ply: unsupported format {fmt}")
+    return fmt, elems, body
 
 
 def read_ply(path):
-    """Inverse of write_ply (binary little-endian, the layout above) -> dict of numpy arrays."""
+    """PLY reader for meshes and point clouds: ascii, binary little- and big-endian; any scalar vertex property type; an
+    optional triangle face list with any integer count and index types (other polygons raise NrwError).  Returns a dict of
+    numpy arrays: vertices [V,3] (x, y, z in their stored type), normals [V,3] or None, colors uint8 [V,3] or None,
+    faces int64 [F,3] (empty without a face element)."""
     with open(path, "rb") as fh:
         data = fh.read()
-    end = data.index(b"end_header\n") + len(b"end_header\n")
-    head = data[:end].decode("ascii").split("\n")
-    nv = int([h for h in head if h.startswith("element vertex")][0].split()[-1])
-    nf = int([h for h in head if h.startswith("element face")][0].split()[-1])
-    props = [h.split()[-1] for h in head if h.startswith("property ") and not h.startswith("property list")]
-    fields = [(p, "<f4" if p in ("x", "y", "z", "nx", "ny", "nz") else "u1") for p in props]
-    v = np.frombuffer(data, dtype=fields, count=nv, offset=end)
-    fc = np.frombuffer(data, dtype=[("n", "u1"), ("i", "<i4", (3,))], count=nf, offset=end + v.nbytes)
-    assert end + v.nbytes + fc.nbytes == len(data) and (fc["n"] == 3).all()
-    out = {"vertices": np.stack([v["x"], v["y"], v["z"]], 1), "normals": np.stack([v["nx"], v["ny"], v["nz"]], 1),
-           "faces": fc["i"].astype(np.int64)}
-    out["colors"] = np.stack([v["red"], v["green"], v["blue"]], 1) if "red" in props else None
-    return out
+    fmt, elems, pos = _ply_header(data)
+    bo = "<" if fmt == "binary_little_endian" else ">"
+    tokens = data[pos:].split() if fmt == "ascii" else None
+    tok = 0
+    vert, faces = None, np.zeros((0, 3), np.int64)
+    for name, count, props in elems:
+        lists = [p for p in props if isinstance(p[1], tuple)]
+        if fmt == "ascii":
+            rows = []
+            for _ in range(count):
+                row = {}
+                for pname, ptype in props:
+                    if isinstance(ptype, tuple):
+                        k = int(tokens[tok])
+                        row[pname] = tokens[tok + 1:tok + 1 + k]
+                        tok += 1 + k
+                    else:
+                        row[pname] = tokens[tok]
+                        tok += 1
+                rows.append(row)
+            if name == "face":
+                if len(lists) != 1 or any(len(r[lists[0][0]]) != 3 for r in rows):
+                    raise NrwError("read_ply: only triangle faces are supported")
+                faces = np.array([[int(x) for x in r[lists[0][0]]] for r in rows], np.int64).reshape(-1, 3)
+            elif name == "vertex":
+                vert = {p: np.array([float(r[p]) for r in rows]).astype(t) for p, t in props if not isinstance(t, tuple)}
+            continue
+        if name == "face" and len(lists) == 1:
+            cnt_t, idx_t = lists[0][1][1], lists[0][1][2]
+            # read as if every face were a triangle; the first count that is not 3 sits at its true offset
+            fields = []
+            for p, t in props:
+                if isinstance(t, tuple):
+                    fields += [(p + "__n", bo + cnt_t), (p, bo + idx_t, (3,))]
+                else:
+                    fields.append((p, bo + t))
+            dt = np.dtype(fields)
+            if pos + dt.itemsize * count > len(data):
+                raise NrwError("read_ply: file shorter than its face element (or polygons that are not triangles)")
+            fc = np.frombuffer(data, dtype=dt, count=count, offset=pos)
+            if (fc[lists[0][0] + "__n"] != 3).any():
+                raise NrwError("read_ply: only triangle faces are supported")
+            faces = fc[lists[0][0]].astype(np.int64).reshape(-1, 3)
+            pos += dt.itemsize * count
+            continue
+        if lists:
+            raise NrwError(f"read_ply: list properties are only supported in the face element (element {name})")
+        dt = np.dtype([(p, bo + t) for p, t in props])
+        if pos + dt.itemsize * count > len(data):
+            raise NrwError(f"read_ply: file shorter than its {name} element")
+        arr = np.frombuffer(data, dtype=dt, count=count, offset=pos)
+        pos += dt.itemsize * count
+        if name == "vertex":
+            vert = {p: arr[p].astype(arr[p].dtype.newbyteorder("=")) for p, _ in props}
+    if vert is None or not all(c in vert for c in "xyz"):
+        raise NrwError("read_ply: no vertex element with x, y, z")
+
+    def stack(names):
+        return np.stack([vert[n] for n in names], 1) if all(n in vert for n in names) else None
+
+    colors = stack(("red", "green", "blue"))
+    return {"vertices": stack(("x", "y", "z")), "normals": stack(("nx", "ny", "nz")), "faces": faces,
+            "colors": None if colors is None else colors.astype(np.uint8)}
 
 
 def _sdf_at(renderer, xyz, chunk):
