@@ -298,6 +298,29 @@ NRW_API int nrw_mesh_sample(const double* verts, long long n_verts, const int64_
                             unsigned long long seed, double* out, int64_t* face_id /*nullable*/, int32_t* status,
                             void* scratch, void* stream);
 
+/* ---- mesh depth rasterisation and back-projection (utils/reproj_filter.py; rules in csrc/raster.cu) ----------------
+ * nrw_raster_depth renders the depth of the mesh verts f64 [n_verts,3] (finite), faces int64 [n_faces,3] seen through
+ * world_to_cam (HOST f64 [3,4] row-major, COLMAP axes: z forward, y down) and the pinhole fx, fy, cx, cy into depth f32
+ * [height,width] (the camera z of the nearest hit with znear <= z <= zfar, 0 where nothing is hit).  cull_back = 1 drops
+ * faces whose right-hand normal points away from the camera.  status (device int32[1]) is written by the call: bit 0 = a
+ * face index outside [0, n_verts) (such faces are skipped).  scratch: nrw_raster_scratch_bytes(n_verts, n_faces, height,
+ * width), 256-byte aligned.  Needs FLT_MIN <= znear <= zfar <= FLT_MAX, fx, fy > 0, height * width <= INT32_MAX.
+ * nrw_reproject_mark back-projects every pixel with depth > 0 from its integer coordinate (c, r) through the pinhole
+ * and cam_to_world (HOST f64 [3,4]) and sets visible[i] = 1 (uint8 [n_ref], not cleared) for the nearest point i of an
+ * nrw_nn_build index over n_ref points when its distance is < threshold.  n_valid (device int64[1], nullable) is
+ * increased by the number of pixels with depth > 0.  scratch: nrw_reproject_scratch_bytes(height, width), 256-byte
+ * aligned.  Neither call reads anything back to the host.  The *_bytes functions return a negative nrw_status for
+ * sizes outside their range. */
+NRW_API long long nrw_raster_scratch_bytes(long long n_verts, long long n_faces, int height, int width);
+NRW_API int nrw_raster_depth(const double* verts, long long n_verts, const int64_t* faces, long long n_faces,
+                             const double* world_to_cam, double fx, double fy, double cx, double cy, int height, int width,
+                             double znear, double zfar, int cull_back, float* depth, int32_t* status, void* scratch,
+                             void* stream);
+NRW_API long long nrw_reproject_scratch_bytes(int height, int width);
+NRW_API int nrw_reproject_mark(const float* depth, int height, int width, double fx, double fy, double cx, double cy,
+                               const double* cam_to_world, const void* index, long long n_ref, double threshold,
+                               uint8_t* visible, long long* n_valid /*nullable*/, void* scratch, void* stream);
+
 /* ---- unit-test hooks ---------------------------------------------------------------------- */
 /* D[M,N] = (sum planes of A)[M,K] * (sum planes of B)[N,K]^T from fp32 inputs: splits into planes in
  * scratch (caller-provided, nrw_gemm_test_scratch_bytes) and runs the selected backend. */

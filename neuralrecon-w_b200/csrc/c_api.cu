@@ -360,6 +360,27 @@ int nrw_mesh_sample(const double* verts, long long n_verts, const int64_t* faces
   NRW_GUARD_END
 }
 
+long long nrw_raster_scratch_bytes(long long n_verts, long long n_faces, int height, int width) {
+  return raster_scratch_bytes(n_verts, n_faces, height, width);
+}
+int nrw_raster_depth(const double* verts, long long n_verts, const int64_t* faces, long long n_faces, const double* world_to_cam,
+                     double fx, double fy, double cx, double cy, int height, int width, double znear, double zfar, int cull_back,
+                     float* depth, int32_t* status, void* scratch, void* stream) {
+  NRW_GUARD_BEGIN
+  return raster_depth(verts, n_verts, faces, n_faces, world_to_cam, fx, fy, cx, cy, height, width, znear, zfar, cull_back, depth,
+                      status, scratch, S(stream));
+  NRW_GUARD_END
+}
+long long nrw_reproject_scratch_bytes(int height, int width) { return reproject_scratch_bytes(height, width); }
+int nrw_reproject_mark(const float* depth, int height, int width, double fx, double fy, double cx, double cy,
+                       const double* cam_to_world, const void* index, long long n_ref, double threshold, uint8_t* visible,
+                       long long* n_valid, void* scratch, void* stream) {
+  NRW_GUARD_BEGIN
+  return reproject_mark(depth, height, width, fx, fy, cx, cy, cam_to_world, index, n_ref, threshold, visible, n_valid, scratch,
+                        S(stream));
+  NRW_GUARD_END
+}
+
 long long nrw_gemm_test_scratch_bytes(int M, int N, int K) {
   const long long a = round_up((long long)M * K, 512), b = round_up((long long)N * K, 512);
   return (a + b) * 3 * 2 + 4096;

@@ -35,28 +35,14 @@
 //    rounds up to total is moved to the next double below it.
 //  * Point: r = sqrt(u_1), a = 1 - r, b = r * (1 - u_2), c = r * u_2, p = (a*v0 + b*v1) + c*v2 per coordinate, each step
 //    _rn.  Samples depend only on (seed, s); nothing is written when the status is non-zero.
-#include <cub/cub.cuh>
-
-#include "octree.h"
+#include "nnsearch.cuh"
 
 namespace nrw {
 
-typedef unsigned long long u64;
-
-static constexpr int NN_LEAF = 32;      // sorted points per leaf
-static constexpr int NN_STACK = 32;     // >= tree depth (26 for 2^31 points)
 static constexpr int NN_THREADS = 128;
 static constexpr int MS_TILE = 1024;    // faces per sequential prefix tile
 
-static inline long long a256(long long x) { return (x + 255) / 256 * 256; }
-
-// ---- shared device arithmetic ---------------------------------------------------------------------------------------
-__device__ __forceinline__ double d2_rn(double dx, double dy, double dz) {
-  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-}
-__device__ __forceinline__ double gap_rn(double q, double lo, double hi) {
-  return q < lo ? __dsub_rn(lo, q) : (q > hi ? __dsub_rn(q, hi) : 0.0);
-}
+// ---- shared device arithmetic (d2_rn, gap_rn and the index layout live in nnsearch.cuh) ----------------------------
 // order-preserving map of doubles to u64 (for atomicMin / atomicMax)
 __device__ __forceinline__ u64 ord_enc(double x) {
   const u64 b = (u64)__double_as_longlong(x);
@@ -89,46 +75,6 @@ __device__ __forceinline__ u64 morton63(double x, double y, double z, const u64*
 }
 
 // ---- nearest-neighbour index ----------------------------------------------------------------------------------------
-struct NnIndex {
-  u64* box_enc;      // [6] reference bounding box, ordered-encoded
-  double* pts;       // [n,3] points in key order
-  int32_t* ord;      // [n] original index of each sorted point
-  double* box;       // [2P,6] node boxes lo xyz, hi xyz (node 0 unused)
-  u64* k0; u64* k1;  // build scratch: keys
-  int32_t* i0;       // build scratch: identity indices
-  void* cub; size_t cub_bytes;
-  long long P, total;
-};
-
-static long long pow2_leaves(long long n) {
-  const long long L = (n + NN_LEAF - 1) / NN_LEAF;
-  long long P = 1;
-  while (P < L) P <<= 1;
-  return P;
-}
-
-static NnIndex nn_layout(void* base, long long n) {
-  NnIndex x;
-  size_t cb = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, cb, (const u64*)nullptr, (u64*)nullptr, (const int32_t*)nullptr, (int32_t*)nullptr,
-                                  (int)n, 0, 63);
-  x.cub_bytes = cb;
-  x.P = pow2_leaves(n);
-  char* p = reinterpret_cast<char*>(base);
-  long long off = 0;
-  auto carve = [&](long long bytes) { char* r = p ? p + off : nullptr; off += a256(bytes); return r; };
-  x.box_enc = reinterpret_cast<u64*>(carve(6 * 8));
-  x.pts = reinterpret_cast<double*>(carve(n * 24));
-  x.ord = reinterpret_cast<int32_t*>(carve(n * 4));
-  x.box = reinterpret_cast<double*>(carve(2 * x.P * 48));
-  x.k0 = reinterpret_cast<u64*>(carve(n * 8));
-  x.k1 = reinterpret_cast<u64*>(carve(n * 8));
-  x.i0 = reinterpret_cast<int32_t*>(carve(n * 4));
-  x.cub = carve((long long)cb);
-  x.total = off;
-  return x;
-}
-
 __global__ void __launch_bounds__(256) nn_bbox_kernel(const double* __restrict__ ref, long long n, u64* __restrict__ enc) {
   double lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -201,10 +147,6 @@ __global__ void nn_level_kernel(long long first, double* __restrict__ box) {
   }
 }
 
-__device__ __forceinline__ double box_d2(const double* __restrict__ b, double qx, double qy, double qz) {
-  return d2_rn(gap_rn(qx, __ldg(b), __ldg(b + 3)), gap_rn(qy, __ldg(b + 1), __ldg(b + 4)), gap_rn(qz, __ldg(b + 2), __ldg(b + 5)));
-}
-
 __global__ void __launch_bounds__(NN_THREADS) nn_query_kernel(const double* __restrict__ pts, const int32_t* __restrict__ ord,
                                                               const double* __restrict__ box, long long n, long long P,
                                                               const double* __restrict__ queries, long long m,
@@ -214,59 +156,11 @@ __global__ void __launch_bounds__(NN_THREADS) nn_query_kernel(const double* __re
   if (t >= m) return;
   const long long qi = qorder[t];
   const double qx = __ldg(queries + 3 * qi), qy = __ldg(queries + 3 * qi + 1), qz = __ldg(queries + 3 * qi + 2);
-  double best = INFINITY;
-  int best_i = 0x7FFFFFFF;
-  int st_node[NN_STACK];
-  double st_d[NN_STACK];
-  int sp = 0, node = 1;
-  const int Pi = (int)P;
-  while (true) {
-    bool descend = false;
-    if (node >= Pi) {
-      const long long s = (long long)(node - Pi) * NN_LEAF, e = s + NN_LEAF < n ? s + NN_LEAF : n;
-      for (long long j = s; j < e; ++j) {
-        const double d2 = d2_rn(__dsub_rn(qx, __ldg(pts + 3 * j)), __dsub_rn(qy, __ldg(pts + 3 * j + 1)),
-                                __dsub_rn(qz, __ldg(pts + 3 * j + 2)));
-        const int oi = __ldg(ord + j);
-        if (d2 < best || (d2 == best && oi < best_i)) {
-          best = d2;
-          best_i = oi;
-        }
-      }
-    } else {
-      const int c0 = 2 * node, c1 = c0 + 1;
-      const double d0 = box_d2(box + 6ll * c0, qx, qy, qz), d1 = box_d2(box + 6ll * c1, qx, qy, qz);
-      const bool first0 = d0 <= d1;
-      const int nn = first0 ? c0 : c1, fn = first0 ? c1 : c0;
-      const double nd = first0 ? d0 : d1, fd = first0 ? d1 : d0;
-      if (fd <= best) {
-        st_node[sp] = fn;
-        st_d[sp] = fd;
-        ++sp;
-      }
-      if (nd <= best) {
-        node = nn;
-        descend = true;
-      }
-    }
-    if (descend) continue;
-    while (sp > 0) {
-      --sp;
-      if (st_d[sp] <= best) {
-        node = st_node[sp];
-        descend = true;
-        break;
-      }
-    }
-    if (!descend) break;
-  }
+  double best;
+  int best_i;
+  nn_nearest(pts, ord, box, n, P, qx, qy, qz, best, best_i);
   dist[qi] = __dsqrt_rn(best);
   idx[qi] = best_i;
-}
-
-static int nn_check_n(long long n, const char* who, const char* what, long long lo) {
-  NRW_CHECK(n >= lo && n <= 0x7FFFFFFFll, NRW_ERR_ARG, "%s: %s = %lld outside [%lld, INT32_MAX]", who, what, n, lo);
-  return NRW_OK;
 }
 
 long long nn_index_bytes(long long n_ref) {

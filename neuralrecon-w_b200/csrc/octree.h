@@ -61,3 +61,15 @@ long long mesh_sample_scratch_bytes(long long n_faces);
 int mesh_sample(const double* verts, long long n_verts, const int64_t* faces, long long n_faces, long long n_samples,
                 unsigned long long seed, double* out, int64_t* face_id, int32_t* status, void* scratch, cudaStream_t s);
 }  // namespace nrw
+
+// mesh depth rasterisation and depth back-projection onto an nn index (raster.cu)
+namespace nrw {
+long long raster_scratch_bytes(long long n_verts, long long n_faces, int height, int width);
+int raster_depth(const double* verts, long long n_verts, const int64_t* faces, long long n_faces, const double* world_to_cam,
+                 double fx, double fy, double cx, double cy, int height, int width, double znear, double zfar, int cull_back,
+                 float* depth, int32_t* status, void* scratch, cudaStream_t s);
+long long reproject_scratch_bytes(int height, int width);
+int reproject_mark(const float* depth, int height, int width, double fx, double fy, double cx, double cy,
+                   const double* cam_to_world, const void* index, long long n_ref, double threshold, uint8_t* visible,
+                   long long* n_valid, void* scratch, cudaStream_t s);
+}  // namespace nrw

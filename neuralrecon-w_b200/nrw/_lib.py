@@ -114,6 +114,12 @@ def lib():
     L.nrw_mesh_sample_scratch_bytes.restype = ll
     L.nrw_mesh_sample_scratch_bytes.argtypes = [ll]
     L.nrw_mesh_sample.argtypes = [vp, ll, vp, ll, ll, C.c_ulonglong, vp, vp, vp, vp, vp]
+    L.nrw_raster_scratch_bytes.restype = ll
+    L.nrw_raster_scratch_bytes.argtypes = [ll, ll, i32, i32]
+    L.nrw_raster_depth.argtypes = [vp, ll, vp, ll, C.POINTER(f64), f64, f64, f64, f64, i32, i32, f64, f64, i32, vp, vp, vp, vp]
+    L.nrw_reproject_scratch_bytes.restype = ll
+    L.nrw_reproject_scratch_bytes.argtypes = [i32, i32]
+    L.nrw_reproject_mark.argtypes = [vp, i32, i32, f64, f64, f64, f64, C.POINTER(f64), vp, ll, f64, vp, vp, vp, vp]
     L.nrw_gemm_test_scratch_bytes.restype = ll
     L.nrw_gemm_test_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_gemm_test.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp]
@@ -135,7 +141,8 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_grid_points_dense", "nrw_grid_points_sparse", "nrw_threshold_compact", "nrw_ctx_set_backward_gate_planes",
            "nrw_mc_scratch_bytes", "nrw_mc_count", "nrw_mc_emit",
            "nrw_nn_index_bytes", "nrw_nn_build", "nrw_nn_query_scratch_bytes", "nrw_nn_query", "nrw_mesh_sample_scratch_bytes",
-           "nrw_mesh_sample"]
+           "nrw_mesh_sample", "nrw_raster_scratch_bytes", "nrw_raster_depth", "nrw_reproject_scratch_bytes",
+           "nrw_reproject_mark"]
 
 
 def check(status, what=""):

@@ -228,12 +228,12 @@ class Mesh:
         write_ply(path, self.vertices, self.faces, self.vertex_normals, self.vertex_colors)
 
 
-def write_ply(path, vertices, faces=None, normals=None, colors=None):
-    """Binary little-endian PLY: vertex x y z [nx ny nz] (float32) [red green blue (uchar)], and with `faces` a face list
-    uchar int.  faces=None and normals=None write a point cloud."""
+def write_ply(path, vertices, faces=None, normals=None, colors=None, double=False):
+    """Binary little-endian PLY: vertex x y z [nx ny nz] (float32, or float64 with double=True) [red green blue (uchar)],
+    and with `faces` a face list uchar int.  faces=None and normals=None write a point cloud."""
     n = len(vertices)
     names = ["x", "y", "z"] + (["nx", "ny", "nz"] if normals is not None else [])
-    fields = [(name, "<f4") for name in names]
+    fields = [(name, "<f8" if double else "<f4") for name in names]
     if colors is not None:
         fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
     v = np.empty(n, dtype=fields)
@@ -245,7 +245,7 @@ def write_ply(path, vertices, faces=None, normals=None, colors=None):
         for c, name in enumerate(("red", "green", "blue")):
             v[name] = colors[:, c]
     head = ["ply", "format binary_little_endian 1.0", f"element vertex {n}"]
-    head += [f"property float {name}" for name in names]
+    head += [f"property {'double' if double else 'float'} {name}" for name in names]
     if colors is not None:
         head += [f"property uchar {name}" for name in ("red", "green", "blue")]
     if faces is not None:
