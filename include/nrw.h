@@ -321,6 +321,54 @@ NRW_API int nrw_reproject_mark(const float* depth, int height, int width, double
                                const double* cam_to_world, const void* index, long long n_ref, double threshold,
                                uint8_t* visible, long long* n_valid /*nullable*/, void* scratch, void* stream);
 
+/* ---- training ray-cache generation (datasets/phototourism.py::read_meta; rules in csrc/raygen.cu) -------------------
+ * nrw_raygen_image writes one image's cache rows: rows f32 [out_cap, 12] (o3, d3, near, far, ts, label, depth, weight;
+ * 11 columns without the label when with_label = 0) and rgbs f32 [out_cap, 3], the kept pixels in raster order, then the
+ * depth_percent padding and a seeded permutation.  Inputs: rgb8 uint8 [height, width, 3]; semantic f32
+ * [sem_height, sem_width] (with_label only); the image's keypoints xys f64 [n_keypoints, 2] (full-resolution pixels) and
+ * point3d_ids int64 [n_keypoints] (-1 = none); the point table point_xyz f64 [n_points, 3] and point_error f64 [n_points]
+ * indexed by point3D id.  counts (device int64[4]) = {rows written, kept rows, depth-valid kept rows, padding rows};
+ * status (device int32[1]): bit 0 = a point3D id past the table, bit 1 = out_cap too small for the padding.  out_cap >=
+ * nrw_raygen_capacity(height, width, depth_percent); scratch: nrw_raygen_scratch_bytes, 256-byte aligned.  Nothing is
+ * read back to the host; the caller reads counts[0] to size its copy.
+ * nrw_depth_range writes, for every image i of w2c f64 [n_images, 3, 4] (device), out f64 [n_images, 2] =
+ * np.percentile(z, (q_lo, q_hi)) of the camera z of the points xyz f64 [n_points, 3] with z > 0, n_front int64
+ * [n_images] (nullable) = their count; status bit 0 = an image with no point in front.  n_points * n_images <=
+ * INT32_MAX; scratch: nrw_depth_range_scratch_bytes.  nrw_raygen_capacity and the *_bytes functions return a negative
+ * nrw_status for sizes, or a depth_percent outside [0, 1), out of range. */
+typedef struct {
+  const uint8_t* octree; /* device: breadth-first child masks */
+  const int32_t* prefix; /* device: exclusive popcount sum */
+  int level;             /* 1..16 */
+  float scene_origin[3]; /* fp32, SfM frame */
+  float scale;           /* > 0 */
+} nrw_octree_ref;
+typedef struct {
+  int height, width;       /* image after the downscale */
+  int img_downscale;       /* >= 1: keypoints are divided by it, the semantic map is read at size // it */
+  float fx, fy, cx, cy;    /* K of the downscaled image, finite, fx, fy != 0 */
+  float c2w[12];           /* fp32 [3,4] row-major, columns 1:2 negated (read_meta) */
+  double w2c_z[4];         /* fp64 third row of COLMAP's [R | t] */
+  int image_id;            /* ts column and the padding stream */
+  int with_label, sem_height, sem_width;
+  int use_voxel;           /* 1: near/far and the kept set from the two octrees; 0: constant near/far, every row kept */
+  float near, far;         /* use_voxel = 0 */
+  float voxel_size;        /* added to the expanded octree's far */
+  nrw_octree_ref sfm;      /* expand 1, radius 1: decides which rows are kept */
+  nrw_octree_ref expanded; /* expand 2, radius 1.5: the stored near/far */
+  double depth_percent;    /* [0, 1) */
+  unsigned long long seed;
+} nrw_raygen_cfg;
+NRW_API long long nrw_raygen_capacity(int height, int width, double depth_percent);
+NRW_API long long nrw_raygen_scratch_bytes(int height, int width, int with_label, long long n_keypoints, long long out_cap);
+NRW_API int nrw_raygen_image(const nrw_raygen_cfg* cfg, const uint8_t* rgb8, const float* semantic, const double* xys,
+                             const int64_t* point3d_ids, long long n_keypoints, const double* point_xyz,
+                             const double* point_error, long long n_points, float* rows, float* rgbs, long long out_cap,
+                             int64_t* counts, int32_t* status, void* scratch, void* stream);
+NRW_API long long nrw_depth_range_scratch_bytes(long long n_points, int n_images);
+NRW_API int nrw_depth_range(const double* xyz, long long n_points, const double* w2c, int n_images, double q_lo, double q_hi,
+                            double* out, int64_t* n_front, int32_t* status, void* scratch, void* stream);
+
 /* ---- unit-test hooks ---------------------------------------------------------------------- */
 /* D[M,N] = (sum planes of A)[M,K] * (sum planes of B)[N,K]^T from fp32 inputs: splits into planes in
  * scratch (caller-provided, nrw_gemm_test_scratch_bytes) and runs the selected backend. */

@@ -381,6 +381,30 @@ int nrw_reproject_mark(const float* depth, int height, int width, double fx, dou
   NRW_GUARD_END
 }
 
+long long nrw_raygen_capacity(int height, int width, double depth_percent) {
+  return raygen_capacity(height, width, depth_percent);
+}
+long long nrw_raygen_scratch_bytes(int height, int width, int with_label, long long n_keypoints, long long out_cap) {
+  return raygen_scratch_bytes(height, width, with_label, n_keypoints, out_cap);
+}
+int nrw_raygen_image(const nrw_raygen_cfg* cfg, const uint8_t* rgb8, const float* semantic, const double* xys,
+                     const int64_t* point3d_ids, long long n_keypoints, const double* point_xyz, const double* point_error,
+                     long long n_points, float* rows, float* rgbs, long long out_cap, int64_t* counts, int32_t* status,
+                     void* scratch, void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(cfg != nullptr, NRW_ERR_ARG, "nrw_raygen_image: null cfg");
+  return raygen_image(*cfg, rgb8, semantic, xys, point3d_ids, n_keypoints, point_xyz, point_error, n_points, rows, rgbs, out_cap,
+                      counts, status, scratch, S(stream));
+  NRW_GUARD_END
+}
+long long nrw_depth_range_scratch_bytes(long long n_points, int n_images) { return depth_range_scratch_bytes(n_points, n_images); }
+int nrw_depth_range(const double* xyz, long long n_points, const double* w2c, int n_images, double q_lo, double q_hi, double* out,
+                    int64_t* n_front, int32_t* status, void* scratch, void* stream) {
+  NRW_GUARD_BEGIN
+  return depth_range(xyz, n_points, w2c, n_images, q_lo, q_hi, out, n_front, status, scratch, S(stream));
+  NRW_GUARD_END
+}
+
 long long nrw_gemm_test_scratch_bytes(int M, int N, int K) {
   const long long a = round_up((long long)M * K, 512), b = round_up((long long)N * K, 512);
   return (a + b) * 3 * 2 + 4096;

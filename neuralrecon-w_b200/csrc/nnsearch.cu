@@ -245,14 +245,6 @@ int nn_query(const void* index, long long n, const double* queries, long long m,
 }
 
 // ---- surface sampling -----------------------------------------------------------------------------------------------
-__device__ __forceinline__ double uniform53(u64 seed, u64 ctr) {
-  u64 z = seed + ctr * 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  z ^= z >> 31;
-  return (double)(z >> 11) * 0x1.0p-53;
-}
-
 // one thread per tile: face areas, sequential inclusive sum inside the tile, the tile's total
 __global__ void ms_area_kernel(const double* __restrict__ v, long long nv, const int64_t* __restrict__ f, long long nf,
                                double* __restrict__ prefix, double* __restrict__ tile_tot, int32_t* __restrict__ status) {

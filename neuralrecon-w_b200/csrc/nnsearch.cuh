@@ -1,5 +1,5 @@
-// Shared pieces of the exact fp64 nearest-neighbour search (rules in nnsearch.cu's header comment): the index layout
-// and the per-query traversal, so every kernel that queries an nrw_nn_build index (nnsearch.cu's nn_query_kernel,
+// Shared pieces of the exact fp64 nearest-neighbour search (rules in nnsearch.cu's header comment): the index layout,
+// the splitmix64 stream and the per-query traversal, so every kernel that queries an nrw_nn_build index (nnsearch.cu's nn_query_kernel,
 // raster.cu's back-projection) runs the same search.
 #pragma once
 #include <cub/cub.cuh>
@@ -14,6 +14,16 @@ static constexpr int NN_LEAF = 32;      // sorted points per leaf
 static constexpr int NN_STACK = 32;     // >= tree depth (26 for 2^31 points)
 
 static inline long long a256(long long x) { return (x + 255) / 256 * 256; }
+
+// the ctr-th output of a splitmix64 stream seeded with `seed` (also the ray-cache padding streams of raygen.cu)
+__host__ __device__ __forceinline__ u64 splitmix64_at(u64 seed, u64 ctr) {
+  u64 z = seed + ctr * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+// 53-bit uniform in [0, 1) from that output
+__device__ __forceinline__ double uniform53(u64 seed, u64 ctr) { return (double)(splitmix64_at(seed, ctr) >> 11) * 0x1.0p-53; }
 
 __device__ __forceinline__ double d2_rn(double dx, double dy, double dz) {
   return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));

@@ -6,44 +6,11 @@
 // sum (children of node i start at hierarchy index 1 + prefix[i]), `pyramid[1][l]` = first hierarchy
 // index of level l.  One thread walks one ray depth-first; a voxel is reported iff the slab test below
 // passes for it AND for all of its ancestors - a pure function of (ray, voxel), so the hit SET does not
-// depend on traversal order and is bit-reproducible against oracle/octree_port.py.
-#include "../../include/nrw_math.h"
-#include "octree.h"
+// depend on traversal order and is bit-reproducible against oracle/octree_port.py.  The traversal lives in
+// octree_trace.cuh, shared with the ray-cache pass (raygen.cu).
+#include "octree_trace.cuh"
 
 namespace nrw {
-
-struct RayN { float o[3], d[3]; };
-
-__device__ __forceinline__ RayN normalise_ray(const float* ro, const float* rd, int r, float ox, float oy, float oz,
-                                              float scale) {
-  RayN q;
-  const float so[3] = {ox, oy, oz};
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    q.d[a] = NRW_ADD(rd[r * 3 + a], 1e-7f);                                   // generate_voxel.py:332
-    q.o[a] = NRW_DIV(NRW_SUB(NRW_ADD(ro[r * 3 + a], 1e-7f), so[a]), scale);   // :333,345
-  }
-  return q;
-}
-
-// slab test against the voxel (x,y,z) of `level`; returns entry depth (>= 0) or -1 when missed
-__device__ __forceinline__ float slab(const RayN& q, int x, int y, int z, int level) {
-  const float r = 1.0f / (float)(1 << level);
-  const int p[3] = {x, y, z};
-  float tmin = -INFINITY, tmax = INFINITY;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const float c = NRW_SUB(NRW_MUL(r, (float)(2 * p[a] + 1)), 1.0f);
-    const float t1 = NRW_DIV(NRW_SUB(NRW_SUB(c, r), q.o[a]), q.d[a]);
-    const float t2 = NRW_DIV(NRW_SUB(NRW_ADD(c, r), q.o[a]), q.d[a]);
-    tmin = fmaxf(tmin, fminf(t1, t2));
-    tmax = fminf(tmax, fmaxf(t1, t2));
-  }
-  if (!(tmax >= tmin) || !(tmax >= 0.0f)) return -1.0f;
-  return fmaxf(tmin, 0.0f);
-}
-
-static constexpr int MAX_LEVEL = 16;
 
 // mode 0: near/far/pid/count.  mode 1: write the hit list at offsets[r] and sort it front-to-back.
 template <int MODE>
@@ -56,48 +23,22 @@ __global__ void octree_trace_kernel(const uint8_t* __restrict__ octree, const in
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= R) return;
   const RayN q = normalise_ray(ro, rd, r, ox, oy, oz, scale);
-  int node[MAX_LEVEL + 1], child[MAX_LEVEL + 1], cx[MAX_LEVEL + 1], cy[MAX_LEVEL + 1], cz[MAX_LEVEL + 1];
-  float tn = INFINITY, tf = -INFINITY;
-  int best = -1, n_hit = 0;
-  const long long base = MODE == 1 ? offsets[r] : 0;
-  int l = 0;
-  node[0] = 0; child[0] = 0; cx[0] = cy[0] = cz[0] = 0;
-  if (slab(q, 0, 0, 0, 0) < 0.0f) l = -1;
-  while (l >= 0) {
-    if (child[l] >= 8) { --l; continue; }
-    const int j = child[l]++;
-    const uint8_t byte = octree[node[l]];
-    if (!((byte >> j) & 1)) continue;
-    const int nx = cx[l] * 2 + ((j >> 2) & 1), ny = cy[l] * 2 + ((j >> 1) & 1), nz = cz[l] * 2 + (j & 1);
-    const float t = slab(q, nx, ny, nz, l + 1);
-    if (t < 0.0f) continue;
-    const int idx = 1 + prefix[node[l]] + __popc((unsigned)byte & ((1u << j) - 1u));
-    if (l + 1 == level) {
-      if (MODE == 0) {
-        if (t < tn || (t == tn && idx < best)) { tn = t; best = idx; }
-        if (t > tf) tf = t;
-      } else {
-        ray_index[base + n_hit] = r;
-        point_index[base + n_hit] = idx;
-        depth[base + n_hit] = t;
-      }
-      ++n_hit;
-    } else {
-      ++l;
-      node[l] = idx; child[l] = 0; cx[l] = nx; cy[l] = ny; cz[l] = nz;
-    }
-  }
   (void)leaf_base;
   if (MODE == 0) {
-    // post-processing of get_near_far (generate_voxel.py:393-400,437-439)
-    float nr = n_hit ? tn : 0.0f, fr = n_hit ? tf : 0.0f;
-    int pd = n_hit ? best : -1;
-    if (!(nr > 1e-4f)) { nr = 0.0f; fr = 0.0f; pd = -1; }
-    near[r] = NRW_MUL(nr, scale);
-    far[r] = NRW_MUL(fr, scale);
-    pid[r] = pd;
-    count[r] = n_hit;
+    const NearFar nf = octree_near_far_ray(octree, prefix, level, q, scale);
+    near[r] = nf.near;
+    far[r] = nf.far;
+    pid[r] = nf.pid;
+    count[r] = nf.count;
   } else {
+    const long long base = offsets[r];
+    int n_hit = 0;
+    octree_walk(octree, prefix, level, q, [&](float t, int idx) {
+      ray_index[base + n_hit] = r;
+      point_index[base + n_hit] = idx;
+      depth[base + n_hit] = t;
+      ++n_hit;
+    });
     // insertion sort by (depth, point index): front-to-back, Morton order on ties
     for (int i = 1; i < n_hit; ++i) {
       const float dk = depth[base + i];

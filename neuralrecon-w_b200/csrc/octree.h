@@ -73,3 +73,15 @@ int reproject_mark(const float* depth, int height, int width, double fx, double 
                    const double* cam_to_world, const void* index, long long n_ref, double threshold, uint8_t* visible,
                    long long* n_valid, void* scratch, cudaStream_t s);
 }  // namespace nrw
+
+// training ray-cache generation: the per-image pass and the per-image near/far percentiles (raygen.cu)
+namespace nrw {
+long long raygen_capacity(int height, int width, double depth_percent);
+long long raygen_scratch_bytes(int height, int width, int with_label, long long n_keypoints, long long out_cap);
+int raygen_image(const nrw_raygen_cfg& cfg, const uint8_t* rgb8, const float* semantic, const double* xys, const int64_t* ids,
+                 long long n_keypoints, const double* xyz, const double* err, long long n_points, float* rows, float* rgbs,
+                 long long out_cap, int64_t* counts, int32_t* status, void* scratch, cudaStream_t s);
+long long depth_range_scratch_bytes(long long n_points, int n_images);
+int depth_range(const double* xyz, long long n_points, const double* w2c, int n_images, double q_lo, double q_hi, double* out,
+                int64_t* n_front, int32_t* status, void* scratch, cudaStream_t s);
+}  // namespace nrw

@@ -47,6 +47,19 @@ class RenderGrads(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in _GRAD_FIELDS]
 
 
+class OctreeRef(C.Structure):
+    _fields_ = [("octree", C.c_void_p), ("prefix", C.c_void_p), ("level", C.c_int), ("scene_origin", C.c_float * 3),
+                ("scale", C.c_float)]
+
+
+class RaygenCfg(C.Structure):
+    _fields_ = [("height", C.c_int), ("width", C.c_int), ("img_downscale", C.c_int), ("fx", C.c_float), ("fy", C.c_float),
+                ("cx", C.c_float), ("cy", C.c_float), ("c2w", C.c_float * 12), ("w2c_z", C.c_double * 4),
+                ("image_id", C.c_int), ("with_label", C.c_int), ("sem_height", C.c_int), ("sem_width", C.c_int),
+                ("use_voxel", C.c_int), ("near", C.c_float), ("far", C.c_float), ("voxel_size", C.c_float),
+                ("sfm", OctreeRef), ("expanded", OctreeRef), ("depth_percent", C.c_double), ("seed", C.c_ulonglong)]
+
+
 _lib = None
 
 
@@ -120,6 +133,14 @@ def lib():
     L.nrw_reproject_scratch_bytes.restype = ll
     L.nrw_reproject_scratch_bytes.argtypes = [i32, i32]
     L.nrw_reproject_mark.argtypes = [vp, i32, i32, f64, f64, f64, f64, C.POINTER(f64), vp, ll, f64, vp, vp, vp, vp]
+    L.nrw_raygen_capacity.restype = ll
+    L.nrw_raygen_capacity.argtypes = [i32, i32, f64]
+    L.nrw_raygen_scratch_bytes.restype = ll
+    L.nrw_raygen_scratch_bytes.argtypes = [i32, i32, i32, ll, ll]
+    L.nrw_raygen_image.argtypes = [C.POINTER(RaygenCfg), vp, vp, vp, vp, ll, vp, vp, ll, vp, vp, ll, vp, vp, vp, vp]
+    L.nrw_depth_range_scratch_bytes.restype = ll
+    L.nrw_depth_range_scratch_bytes.argtypes = [ll, i32]
+    L.nrw_depth_range.argtypes = [vp, ll, vp, i32, f64, f64, vp, vp, vp, vp, vp]
     L.nrw_gemm_test_scratch_bytes.restype = ll
     L.nrw_gemm_test_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_gemm_test.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp]
@@ -142,7 +163,8 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_mc_scratch_bytes", "nrw_mc_count", "nrw_mc_emit",
            "nrw_nn_index_bytes", "nrw_nn_build", "nrw_nn_query_scratch_bytes", "nrw_nn_query", "nrw_mesh_sample_scratch_bytes",
            "nrw_mesh_sample", "nrw_raster_scratch_bytes", "nrw_raster_depth", "nrw_reproject_scratch_bytes",
-           "nrw_reproject_mark"]
+           "nrw_reproject_mark", "nrw_raygen_capacity", "nrw_raygen_scratch_bytes", "nrw_raygen_image",
+           "nrw_depth_range_scratch_bytes", "nrw_depth_range"]
 
 
 def check(status, what=""):

@@ -88,10 +88,11 @@ def read_cameras(path):
     return out
 
 
-def read_images(path):
+def read_images(path, with_points=False):
     """images.bin (utils/colmap_utils.py::read_images_binary layout, little endian): u64 count, then per image i32 id,
     4 f64 qvec, 3 f64 tvec, i32 camera id, a NUL-terminated UTF-8 name, u64 point count and that many (f64 x, f64 y,
-    i64 point3D id) records, which are skipped.  Returns {id: Image} in file order."""
+    i64 point3D id) records.  Returns {id: Image} in file order.  The 2-D points are skipped unless with_points, which
+    returns {id: (Image, xys float64 [k,2], point3D_ids int64 [k])} instead."""
     with open(path, "rb") as fh:
         data = fh.read()
     try:
@@ -104,8 +105,17 @@ def read_images(path):
             name = data[off:end].decode("utf-8")
             off = end + 1
             npts = struct.unpack_from("<Q", data, off)[0]
-            off += 8 + 24 * npts
-            out[r[0]] = Image(id=r[0], qvec=np.array(r[1:5]), tvec=np.array(r[5:8]), camera_id=r[8], name=name)
+            off += 8
+            im = Image(id=r[0], qvec=np.array(r[1:5]), tvec=np.array(r[5:8]), camera_id=r[8], name=name)
+            if with_points:
+                if off + 24 * npts > len(data):
+                    raise NrwError(f"read_images: {path} is truncated")
+                rec = np.frombuffer(data, dtype=np.dtype([("x", "<f8"), ("y", "<f8"), ("id", "<i8")]), count=npts, offset=off)
+                xys = np.stack([rec["x"], rec["y"]], 1).astype(np.float64)
+                out[r[0]] = (im, xys, rec["id"].astype(np.int64))
+            else:
+                out[r[0]] = im
+            off += 24 * npts
     except (struct.error, ValueError) as e:
         raise NrwError(f"read_images: {path} is truncated") from e
     if off > len(data):
