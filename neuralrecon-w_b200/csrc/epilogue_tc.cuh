@@ -1,16 +1,14 @@
 // Epilogue of the tensor-core GEMM kernels: one 32-row x 16-column chunk per call.
 //
-// The GEMM hands lane r of a warp ROW r of the accumulator chunk (gemm_tc.cu stages it through shared memory).  Doing the global I/O in
-// that layout would touch 32 different cache lines per instruction, so the chunk is transposed ONCE
-// through a per-warp 2 KB shared staging tile (XOR-swizzled 16-byte slots, conflict-free both ways) into
-// the "line" layout: lane L owns columns 4*(L&3)..+3 of rows (L>>2) + 8*it, it = 0..3.  In that layout
-// every auxiliary load and every store of the epilogue is a direct, sector-aligned global access (8 rows
-// x 64 B per fp32 instruction, 8 rows x 32 B per bf16 instruction) and all arithmetic is elementwise, so
-// nothing else goes through shared memory.
+// The GEMM hands a warp its 32 x 16 accumulator chunk in the "line" layout: lane L owns columns 4*(L&3)..+3 of rows (L>>2) + 8*it,
+// it = 0..3 (gemm_tc.cu reads it that way out of the shared-memory tile it stages the accumulator fragments in).  In that
+// layout every auxiliary load and every store of the epilogue is a direct, sector-aligned global access (8 rows x 64 B per
+// fp32 instruction, 8 rows x 32 B per bf16 instruction) and all arithmetic is elementwise, so nothing else goes through
+// shared memory.
 //
 // This file is the line-layout I/O layer both chunk epilogues use (the generic epi_chunk16 below and the specialised kinds of
-// epilogue_fast.cuh): the transpose, the full-tile accessors, the line accessors with their ragged / unaligned fallbacks, bf16
-// packing and column sums.
+// epilogue_fast.cuh): the full-tile accessors, the line accessors with their ragged / unaligned fallbacks, bf16 packing and
+// column sums.
 #pragma once
 #include "epilogue.cuh"
 
@@ -25,23 +23,6 @@ struct LineLayout {
 
 __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 __device__ __forceinline__ bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
-
-// The one transpose: v = row `lane` of the chunk -> x[4*it + k] = row it*8 + (lane>>2), column 4*(lane&3) + k.
-// stg: this warp's 2 KB tile (64-byte rows, slot' = slot ^ ((row >> 1) & 3)); it may be overwritten again on return.
-__device__ __forceinline__ void line_transpose(float* stg, const float (&v)[16], int lane, float (&x)[16]) {
-  const int sl = lane & 3, r0 = lane >> 2;
-#pragma unroll
-  for (int s = 0; s < 4; ++s)
-    *reinterpret_cast<float4*>(stg + lane * 16 + ((s ^ ((lane >> 1) & 3)) << 2)) = make_float4(v[4 * s], v[4 * s + 1], v[4 * s + 2], v[4 * s + 3]);
-  __syncwarp();
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int rr = it * 8 + r0;
-    const float4 t = *reinterpret_cast<const float4*>(stg + rr * 16 + ((sl ^ ((rr >> 1) & 3)) << 2));
-    x[4 * it] = t.x; x[4 * it + 1] = t.y; x[4 * it + 2] = t.z; x[4 * it + 3] = t.w;
-  }
-  __syncwarp();
-}
 
 // Side-stream loads.  Warps working on neighbouring column chunks of the same rows read NEIGHBOURING 64-byte (fp32) /
 // 32-byte (bf16) pieces of the same rows, so the first of them asks L2 to fetch the whole aligned 256 bytes
@@ -66,13 +47,23 @@ __device__ __forceinline__ void tile_load_f32(const float* p, long long ld, floa
     o[4 * it] = t.x; o[4 * it + 1] = t.y; o[4 * it + 2] = t.z; o[4 * it + 3] = t.w;
   }
 }
-__device__ __forceinline__ void tile_load_bf16(const bf16* p, long long ld, float (&o)[16]) {
+// bf16 tiles can stay packed in registers (8 words for 16 values) until they are used: tile_load_bf16 = raw load + unpack
+__device__ __forceinline__ void tile_load_bf16_raw(const bf16* p, long long ld, uint2 (&r)[4]) {
+#pragma unroll
+  for (int it = 0; it < 4; ++it) r[it] = ldg2u(p + it * 8 * ld);
+}
+__device__ __forceinline__ void unpack_bf16(const uint2 (&r)[4], float (&o)[16]) {
 #pragma unroll
   for (int it = 0; it < 4; ++it) {
-    const uint2 t = ldg2u(p + it * 8 * ld);
+    const uint2 t = r[it];
     o[4 * it] = __uint_as_float(t.x << 16); o[4 * it + 1] = __uint_as_float(t.x & 0xFFFF0000u);
     o[4 * it + 2] = __uint_as_float(t.y << 16); o[4 * it + 3] = __uint_as_float(t.y & 0xFFFF0000u);
   }
+}
+__device__ __forceinline__ void tile_load_bf16(const bf16* p, long long ld, float (&o)[16]) {
+  uint2 r[4];
+  tile_load_bf16_raw(p, ld, r);
+  unpack_bf16(r, o);
 }
 __device__ __forceinline__ void tile_store_f32(float* p, long long ld, const float (&o)[16]) {
 #pragma unroll
@@ -239,10 +230,10 @@ __device__ __forceinline__ void line_colsum_add(const float (&w)[16], int lane, 
   if ((lane & 4) == 0) atomicAdd(cs_tile + (lane & 3) * 4 + (hi16 ? 2 : 0) + (hi8 ? 1 : 0), k);   // shared-memory reduction
 }
 
-// v: row `lane` of the accumulator chunk (columns nc..nc+15 of rows m0w..m0w+31).  stg: this warp's 2 KB tile.
+// x_acc: the accumulator chunk (columns nc..nc+15 of rows m0w..m0w+31) in the line layout.
 // cs_tile: this CTA's shared column-sum accumulator for columns nc..nc+15 (flushed by the kernel); non-null iff e.colsum is set
 // and the epilogue is not atomic.
-__device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const float (&v)[16], int m0w, int nc, int M, int N, int lane,
+__device__ __forceinline__ void epi_chunk16(const Epi& e, const float (&x_acc)[16], int m0w, int nc, int M, int N, int lane,
                                             float* cs_tile) {
   LineLayout L;
   L.rows_valid = min(32, M - m0w);
@@ -253,7 +244,8 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, float* stg, const floa
   L.r0 = lane >> 2;
   L.full = L.rows_valid == 32;
   float x[16];
-  line_transpose(stg, v, lane, x);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) x[i] = x_acc[i];
   // ---- v = acc + bias + rowvec * colvec ----
   if (e.bias) {
     float b[4];

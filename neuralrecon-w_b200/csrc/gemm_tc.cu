@@ -15,8 +15,8 @@
 //   the producer warpgroup (40) to the consumers (232).
 // * one smem ring of TMA stages (128B swizzle), filled in item order, so the loads of the next k-blocks (and of
 //   the next items) overlap the MMAs and the epilogues.  A stage has a single consuming warpgroup.
-// * the epilogue stages a warpgroup's accumulators (one 64-row half at a time) through shared memory into the row
-//   layout the chunk epilogues take (epilogue_tc.cuh / epilogue_fast.cuh: one 32-row x 16-column chunk per warp).
+// * the epilogue stages a warpgroup's accumulators (64 columns of one 64-row half per round) through shared memory into the
+//   line layout the chunk epilogues take (epilogue_tc.cuh / epilogue_fast.cuh: two 32-row x 16-column chunks per warp and round).
 // * mn_major=1 consumes both operands "transposed" straight from their natural row-major
 //   [rows=K][cols=M|N] layout (MN-major wgmma descriptors) - used for weight gradients
 //   dW = dY^T X with split-K over the sample dimension and fp32 atomics in the epilogue.
@@ -40,15 +40,20 @@ static constexpr int MAX_STAGES = 8;
 static constexpr int N_CONSUMER_WARPS = 8;             // two ping-pong warpgroups, each owning whole 128-row tiles
 static constexpr int N_THREADS = 32 * N_CONSUMER_WARPS + 128;   // + the producer warpgroup
 static constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // setmaxnreg split: 128 x 40 + 256 x 232 <= 65536
-static constexpr int EPI_LD = 36;                      // staging row pitch in floats: 32 columns + 4 (16-byte aligned rows)
-static constexpr int EPI_WG_BYTES = 64 * EPI_LD * 4;   // one warpgroup's staging tile [64 rows][32 columns]; doubles as 4 x 2 KB warp tiles
+static constexpr int EPI_COLS = 64;                    // columns per epilogue round; staging rows are unpadded (16-byte slots XOR-swizzled)
+static constexpr int EPI_WG_BYTES = 64 * EPI_COLS * 4; // one warpgroup's staging tile [64 rows][64 columns]
 static constexpr int CS_BYTES = 1024;                  // column-sum accumulators: 128 columns of the current n-tile per warpgroup
 static constexpr int BAR_TURN = 4;                     // named barriers 4 + wg: warpgroup wg's turn at the tensor cores
 static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 32 * N_CONSUMER_WARPS <= 65536, "register file");
 static constexpr int BAR_BYTES = 256;                  // 2 x MAX_STAGES mbarriers
 static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + 2 * EPI_WG_BYTES + CS_BYTES;
 static_assert(SMEM_BYTES <= 232448, "dynamic shared memory limit of sm_90");
-static_assert(4 * 2048 <= EPI_WG_BYTES, "the 2 KB per-warp epilogue tiles live in the warpgroup's staging tile");
+
+// Staging tile: 16-byte slot s of row r is stored at slot s ^ epi_swz(r) of the row.  The XOR permutes the 8 bank groups of a
+// 128-byte wavefront: a half-warp's fragment stores (4 consecutive rows 4k..4k+3 x slots 2j, 2j+1: epi_swz / 2 takes 4
+// different values) and a quarter-warp's line-layout reads (rows 2k, 2k+1 x slots 4c..4c+3: epi_swz differs in bit 2) hit 8
+// different bank groups, so both directions are conflict-free without padding.
+__device__ __forceinline__ int epi_swz(int r) { return ((r & 1) << 2) | (r & 2) | ((r >> 2) & 1); }
 
 struct TcParams {
   CUtensorMap tmA[3];
@@ -296,7 +301,6 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     constexpr uint32_t KSTEP = MN_MAJOR ? (16 * 128) : 32;  // bytes per wgmma K=16
     const uint64_t desc_hi = make_gdesc(0, LBO, SBO);         // everything but the start address
     float* stage_tile = epi_buf + wg * (EPI_WG_BYTES / 4);
-    float* stg = stage_tile + wi * 512;                      // this warp's 2 KB tile (after the staging tile has been read)
     const bool use_cs = p.epi.colsum != nullptr && !p.epi.atomic;
     float* cs_wg = cs_buf + 128 * wg;                        // this warpgroup's column-sum accumulator
     const int ctid = threadIdx.x & 127;
@@ -377,39 +381,53 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       if (kb1 <= kb0) continue;
       NRW_PROF_T0(prof);
       if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6 + po], 1ull);
-      // ---- epilogue, per 64-row half h: 32 columns at a time through the warpgroup's staging tile.  Fragment of warp wi:
+      // ---- epilogue, per 64-row half h: 64 columns per round through the warpgroup's staging tile.  Fragment of warp wi:
       // acc[h][4j + {0,1}] = row 64 h + 16 wi + lane / 4, columns 8 j + 2 (lane % 4) + {0,1}; acc[h][4j + {2,3}] = the same columns
-      // of row + 8.  After the barrier warp wi takes rows 64 h + 32 (wi & 1) .. +31 (row = lane) and columns 16 (wi >> 1) .. +15
-      // of the 32: the chunk layout of epi_chunk16. ----
+      // of row + 8.  After the barrier warp wi reads rows 64 h + 32 (wi & 1) .. +31 and columns 16 (wi >> 1) .. +15 (chunk 0) and
+      // 32 + 16 (wi >> 1) .. +15 (chunk 1) of the round's 64 straight in the line layout of the chunk epilogues (lane L: rows
+      // L / 4 + 8 it, columns 4 (L % 4) .. +3). ----
       const int r0 = 16 * wi + (lane >> 2), c0 = 2 * (lane & 3);
       const int qq = wi & 1, cc = wi >> 1;
-      const int n_cp = (min(BN, p.N - n0) + 31) / 32;
+      const int n_rounds = (min(BN, p.N - n0) + EPI_COLS - 1) / EPI_COLS;
+      float* st_w = stage_tile + r0 * EPI_COLS + (c0 & 3);          // fragment stores: row r0 (r0 + 8 has the same swizzle)
+      const int st_x = (c0 >> 2) ^ epi_swz(r0);                      // slot 2 jj + (c0 >> 2) -> 2 jj ^ st_x
+      const float* st_l = stage_tile + (32 * qq + (lane >> 2)) * EPI_COLS;   // line reads: rows + 8 it share the swizzle
+      const int ln_x = (lane & 3) ^ epi_swz(lane >> 2);              // slot 4 c + (lane & 3) -> 4 c ^ ln_x
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int m0w = m0 + 64 * h + 32 * qq;
         float hacc[4] = {0.0f, 0.0f, 0.0f, 0.0f};   // FWD_HEAD: this lane's rows of the fused SDF-head dot product
 #pragma unroll
-        for (int cp = 0; cp < BN / 32; ++cp) {
-          if (cp >= n_cp) break;                     // warpgroup-uniform
+        for (int rd = 0; rd < BN / EPI_COLS; ++rd) {
+          if (rd >= n_rounds) break;                 // warpgroup-uniform
+          const int nc = n0 + EPI_COLS * rd + 16 * cc;
+          const bool act = nc < p.N && m0w < p.M;    // warp-uniform
+          const bool full = act && pair_full<EK>(p.epi, m0w, nc, p.M, p.N);
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int jf = 4 * cp + jj;
-            *reinterpret_cast<float2*>(stage_tile + r0 * EPI_LD + 8 * jj + c0) = make_float2(acc[h][4 * jf], acc[h][4 * jf + 1]);
-            *reinterpret_cast<float2*>(stage_tile + (r0 + 8) * EPI_LD + 8 * jj + c0) = make_float2(acc[h][4 * jf + 2], acc[h][4 * jf + 3]);
+          for (int jj = 0; jj < 8; ++jj) {
+            const int jf = 8 * rd + jj;
+            float* d = st_w + (((2 * jj) ^ st_x) << 2);
+            *reinterpret_cast<float2*>(d) = make_float2(acc[h][4 * jf], acc[h][4 * jf + 1]);
+            *reinterpret_cast<float2*>(d + 8 * EPI_COLS) = make_float2(acc[h][4 * jf + 2], acc[h][4 * jf + 3]);
           }
+          FastSide f0, f1;                           // issued before the barrier: their latency overlaps its wait
+          if (full) pair_load<EK>(p.epi, m0w, nc, lane, f0, f1);
           named_bar_sync(2 + wg, 128);
-          float v[16];
-          const float* src = stage_tile + (32 * qq + lane) * EPI_LD + 16 * cc;
+          if (act) {
+            float* cs = use_cs ? cs_wg + EPI_COLS * rd + 16 * cc : nullptr;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 t4 = *reinterpret_cast<const float4*>(src + 4 * i);
-            v[4 * i] = t4.x; v[4 * i + 1] = t4.y; v[4 * i + 2] = t4.z; v[4 * i + 3] = t4.w;
+            for (int c = 0; c < 2; ++c) {
+              if (c == 1 && nc + 32 >= p.N) break;   // warp-uniform
+              float x[16];
+#pragma unroll
+              for (int it = 0; it < 4; ++it) {
+                const float4 t = *reinterpret_cast<const float4*>(st_l + it * 8 * EPI_COLS + (((4 * cc + 8 * c) ^ ln_x) << 2));
+                x[4 * it] = t.x; x[4 * it + 1] = t.y; x[4 * it + 2] = t.z; x[4 * it + 3] = t.w;
+              }
+              epi_pair_chunk<EK>(p.epi, x, full, c ? f1 : f0, m0w, nc + 32 * c, p.M, p.N, lane, cs ? cs + 32 * c : nullptr, hacc);
+            }
           }
-          named_bar_sync(2 + wg, 128);               // the staging tile is free: it holds the warps' 2 KB tiles from here on
-          const int nc = n0 + 32 * cp + 16 * cc;
-          if (nc < p.N && m0w < p.M)                 // warp-uniform
-            epi_fast16<EK>(p.epi, stg, v, m0w, nc, p.M, p.N, lane, use_cs ? cs_wg + 32 * cp + 16 * cc : nullptr, hacc);
-          named_bar_sync(2 + wg, 128);
+          named_bar_sync(2 + wg, 128);               // every warp has read the staging tile: the next round may overwrite it
         }
         if (EK == EK_FWD_HEAD && (lane & 3) == 0) { // partial[row][slot], slot = n-tile * 2 + column class: plain stores
           const int slot = (n0 / BN) * 2 + cc;
