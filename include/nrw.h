@@ -369,6 +369,23 @@ NRW_API long long nrw_depth_range_scratch_bytes(long long n_points, int n_images
 NRW_API int nrw_depth_range(const double* xyz, long long n_points, const double* w2c, int n_images, double q_lo, double q_hi,
                             double* out, int64_t* n_front, int32_t* status, void* scratch, void* stream);
 
+/* ---- point-cloud visibility through its voxel octree (utils/kaolin_renderer.py; rules in csrc/voxelvis.cu) -----------
+ * nrw_voxel_cast casts one ray per pixel of a height x width pinhole view (fx, fy, cx, cy in fp32, pixel (c, r) from the
+ * integer grid) from cam_to_world (host f64 [3,4] row-major, rounded to fp32) through an octree of nrw_octree_build
+ * (octree, prefix on the device, pyramid_host [2, level+2] on the host; level 1..16), normalised by scene_origin and
+ * scale as get_near_far does, and takes the first leaf each ray hits.  Outputs, each nullable: visible u8 [n_leaf]
+ * set to 1 at every hit leaf (never cleared, so views accumulate), depth f32 [height, width] = near * scale / |d|
+ * (0 on a miss), leaf i32 [height, width] (-1 on a miss), n_hit (device int64) increased by the number of hit pixels.
+ * nrw_voxel_lookup maps points f64 [n_points, 3], already normalised ((x - origin) / scale), to their leaf index
+ * (-1 outside the open cube (-1, 1)^3); a quantised cell that is not a leaf also gives -1 and sets bit 0 of status
+ * (device int32, cleared first).  Every argument is checked before any launch; nothing is read back to the host. */
+NRW_API int nrw_voxel_cast(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid_host, int level,
+                           const float scene_origin[3], float scale, const double* cam_to_world, float fx, float fy,
+                           float cx, float cy, int height, int width, uint8_t* visible, float* depth, int32_t* leaf,
+                           int64_t* n_hit, void* stream);
+NRW_API int nrw_voxel_lookup(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid_host, int level,
+                             const double* points, long long n_points, int32_t* leaf, int32_t* status, void* stream);
+
 /* ---- unit-test hooks ---------------------------------------------------------------------- */
 /* D[M,N] = (sum planes of A)[M,K] * (sum planes of B)[N,K]^T from fp32 inputs: splits into planes in
  * scratch (caller-provided, nrw_gemm_test_scratch_bytes) and runs the selected backend. */

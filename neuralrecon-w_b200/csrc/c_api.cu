@@ -405,6 +405,22 @@ int nrw_depth_range(const double* xyz, long long n_points, const double* w2c, in
   NRW_GUARD_END
 }
 
+int nrw_voxel_cast(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid_host, int level,
+                   const float scene_origin[3], float scale, const double* cam_to_world, float fx, float fy, float cx,
+                   float cy, int height, int width, uint8_t* visible, float* depth, int32_t* leaf, int64_t* n_hit,
+                   void* stream) {
+  NRW_GUARD_BEGIN
+  return voxel_cast(octree, prefix, pyramid_host, level, scene_origin, scale, cam_to_world, fx, fy, cx, cy, height, width,
+                    visible, depth, leaf, n_hit, S(stream));
+  NRW_GUARD_END
+}
+int nrw_voxel_lookup(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid_host, int level,
+                     const double* points, long long n_points, int32_t* leaf, int32_t* status, void* stream) {
+  NRW_GUARD_BEGIN
+  return voxel_lookup(octree, prefix, pyramid_host, level, points, n_points, leaf, status, S(stream));
+  NRW_GUARD_END
+}
+
 long long nrw_gemm_test_scratch_bytes(int M, int N, int K) {
   const long long a = round_up((long long)M * K, 512), b = round_up((long long)N * K, 512);
   return (a + b) * 3 * 2 + 4096;

@@ -11,8 +11,25 @@ int octree_hits(const uint8_t* octree, const int32_t* prefix, const int32_t* pyr
                 const int64_t* offsets, int32_t* ray_index, int32_t* point_index, float* depth, cudaStream_t s);
 }  // namespace nrw
 
+// point-cloud visibility: first-hit cast per view and point -> leaf lookup (voxelvis.cu)
+namespace nrw {
+int voxel_cast(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid, int level, const float origin[3],
+               float scale, const double* c2w, float fx, float fy, float cx, float cy, int H, int W, uint8_t* visible,
+               float* depth, int32_t* leaf, int64_t* n_hit, cudaStream_t s);
+int voxel_lookup(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid, int level, const double* points,
+                 long long n, int32_t* leaf, int32_t* status, cudaStream_t s);
+}  // namespace nrw
+
 // K0: octree builder (octree_build.cu)
 namespace nrw {
+// quantize_points of one coordinate in fp64 (the reference feeds float64 numpy points): floor(clamp(2^L (x+1)/2, 0,
+// 2^L-1)).  Shared by the builder and the point -> leaf lookup of voxelvis.cu, so both place a point in the same cell.
+__host__ __device__ __forceinline__ unsigned quantize_coord(double x, int level) {
+  const double res = (double)(1 << level);
+  double v = res * (x + 1.0) / 2.0;
+  v = fmin(fmax(v, 0.0), res - 1.0);
+  return (unsigned)floor(v);
+}
 long long octree_build_scratch_bytes(int n_points, int level, int cap_nonleaf);
 int octree_build(const void* points, int is_f64, int n, int level, uint8_t* octree, int32_t* prefix, int32_t* pyramid,
                  int16_t* points_out, int cap_nonleaf, int cap_total, int32_t* counts_out, void* scratch, cudaStream_t s);

@@ -15,20 +15,14 @@ namespace nrw {
 
 typedef unsigned long long u64;
 
-// quantize_points in fp64 (the reference feeds float64 numpy points): floor(clamp(2^L (x+1)/2, 0, 2^L-1));
-// Morton digit = (x&1)<<2 | (y&1)<<1 | (z&1), most significant level first.
+// quantize_coord (octree.h) per axis; Morton digit = (x&1)<<2 | (y&1)<<1 | (z&1), most significant level first.
 template <typename T>
 __global__ void k0_morton_kernel(const T* __restrict__ pts, int n, int level, u64* __restrict__ keys) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double res = (double)(1 << level);
   unsigned q[3];
 #pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    double v = res * ((double)pts[3 * (long long)i + a] + 1.0) / 2.0;
-    v = fmin(fmax(v, 0.0), res - 1.0);
-    q[a] = (unsigned)floor(v);
-  }
+  for (int a = 0; a < 3; ++a) q[a] = quantize_coord((double)pts[3 * (long long)i + a], level);
   u64 m = 0;
   for (int b = 0; b < level; ++b)
     m |= ((u64)((q[0] >> b) & 1u) << (3 * b + 2)) | ((u64)((q[1] >> b) & 1u) << (3 * b + 1)) | ((u64)((q[2] >> b) & 1u) << (3 * b));

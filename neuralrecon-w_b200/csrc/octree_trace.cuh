@@ -86,4 +86,52 @@ __device__ __forceinline__ NearFar octree_near_far_ray(const uint8_t* __restrict
   return NearFar{NRW_MUL(nr, scale), NRW_MUL(fr, scale), pd, n_hit};
 }
 
+struct FirstHit { float near; int pid; };
+
+// The near and pid of octree_near_far_ray (unscaled near; 0 and -1 unless near > 1e-4), found with pruning: children
+// are visited front to back (digit j ^ mask, mask = the ray's sign octant) and a subtree whose slab entry t is strictly
+// greater than the best leaf so far is skipped.  Why that is exact is argued in voxelvis.cu's header.  A ray with a
+// non-finite direction component takes the unpruned walk.
+__device__ __forceinline__ FirstHit octree_first_hit(const uint8_t* __restrict__ octree, const int32_t* __restrict__ prefix,
+                                                     int level, const RayN& q) {
+  float tn = INFINITY;
+  int best = -1;
+  bool hit = false;
+  if (!(isfinite(q.d[0]) && isfinite(q.d[1]) && isfinite(q.d[2]))) {
+    octree_walk(octree, prefix, level, q, [&](float t, int idx) {
+      if (t < tn || (t == tn && idx < best)) { tn = t; best = idx; }
+      hit = true;
+    });
+  } else {
+    const int mask = (q.d[0] < 0.0f ? 4 : 0) | (q.d[1] < 0.0f ? 2 : 0) | (q.d[2] < 0.0f ? 1 : 0);
+    int node[MAX_LEVEL + 1], child[MAX_LEVEL + 1], cx[MAX_LEVEL + 1], cy[MAX_LEVEL + 1], cz[MAX_LEVEL + 1];
+    float te[MAX_LEVEL + 1];
+    int l = 0;
+    node[0] = 0; child[0] = 0; cx[0] = cy[0] = cz[0] = 0;
+    te[0] = slab(q, 0, 0, 0, 0);
+    if (te[0] < 0.0f) l = -1;
+    while (l >= 0) {
+      if (child[l] >= 8 || te[l] > tn) { --l; continue; }
+      const int j = (child[l]++) ^ mask;
+      const uint8_t byte = octree[node[l]];
+      if (!((byte >> j) & 1)) continue;
+      const int nx = cx[l] * 2 + ((j >> 2) & 1), ny = cy[l] * 2 + ((j >> 1) & 1), nz = cz[l] * 2 + (j & 1);
+      const float t = slab(q, nx, ny, nz, l + 1);
+      if (t < 0.0f || t > tn) continue;
+      const int idx = 1 + prefix[node[l]] + __popc((unsigned)byte & ((1u << j) - 1u));
+      if (l + 1 == level) {
+        if (t < tn || (t == tn && idx < best)) { tn = t; best = idx; }
+        hit = true;
+      } else {
+        ++l;
+        node[l] = idx; child[l] = 0; cx[l] = nx; cy[l] = ny; cz[l] = nz; te[l] = t;
+      }
+    }
+  }
+  // the final rule of octree_near_far_ray
+  const float nr = hit ? tn : 0.0f;
+  if (!(nr > 1e-4f)) return FirstHit{0.0f, -1};
+  return FirstHit{nr, hit ? best : -1};
+}
+
 }  // namespace nrw

@@ -10,10 +10,16 @@ is the union over the views: the kept target points as rows [x, y, z, r, g, b] (
 np.unique(axis=0) returns them, written to <output_path>/reprojected.ply with double coordinates.
 
 Deviations from the reference, by design: depth is fp64 (OpenGL has fp32 and a 24-bit depth buffer), nearest neighbours
-are exact with the smallest index on ties, point-cloud sources (its Kaolin octree branch) and --visualize raise NrwError,
-and --n_cpus / --n_gpus are accepted and ignored (one process; the union over views does not depend on the split).
+are exact with the smallest index on ties, --visualize raises NrwError, and --n_cpus / --n_gpus are accepted and ignored
+(one process; the union over views does not depend on the split).
 
-    python -m nrw.reprojection --src_file M.ply --target_file M.ply --data_path SCENE --output_path OUT
+With --point_source the source is a point cloud (its faces, if any, are ignored): the reference's Kaolin branch
+(utils/kaolin_renderer.py).  The source points are voxelised into an octree (nrw.octree.gen_octree, expand 0, in the
+frame of the points), every pixel of every training view casts one ray to the first leaf it hits (csrc/voxelvis.cu), and
+a source point is kept when its leaf was hit by some view; the output rows are the target points of the kept source
+indices, as for meshes.  Deviations of this branch are listed in INTEGRATION.md.
+
+    python -m nrw.reprojection --src_file M.ply --target_file M.ply --data_path SCENE --output_path OUT [--point_source]
 """
 import csv
 import ctypes as C
@@ -28,6 +34,7 @@ from ._lib import NrwError, check, ptr, stream_ptr
 from .colmap import read_cameras, read_images
 from .evaluation import NearestNeighbours, _device, _points, _scratch
 from .mesh import read_ply, write_ply
+from .octree import gen_octree, scene_bbox
 
 # pyrender.constants DEFAULT_Z_NEAR / DEFAULT_Z_FAR, the clip range of its IntrinsicsCamera
 Z_NEAR = 0.05
@@ -206,12 +213,104 @@ def reproj_filter(vertices, faces, target, intrinsics, extrinsics, whs, voxel_si
     return marker.mask()
 
 
-def _sfm2gt(data_path):
+class VoxelRenderer:
+    """First-hit voxel renders of a point cloud [N,3] (utils/kaolin_renderer.py): the points are voxelised once with
+    nrw.octree.gen_octree(scene_config, points, voxel_size, expand=0, in_sfm=False) on the CUDA device.
+    __call__(height, width, intrinsic, world_to_cam) -> (depth float32 [H, W], leaf int32 [H, W]) CUDA tensors: per
+    pixel the first leaf its ray hits (-1 on a miss) and the entry distance divided by the length of the ray's camera
+    direction ((c - cx)/fx, (r - cy)/fy, 1), i.e. the camera z of a rigid camera (0 on a miss); every hit leaf is
+    marked in `visible`, which accumulates over calls.  point_leaves() -> int32 [N] CUDA tensor: each input point's leaf, or -1
+    for a point outside the octree's cube.  Rules in csrc/voxelvis.cu."""
+
+    def __init__(self, points, scene_config, voxel_size, device=0):
+        self.dev = _device(device)
+        self.points = _points(points, "VoxelRenderer", self.dev)
+        voxel_size = float(voxel_size)
+        if not (np.isfinite(voxel_size) and voxel_size > 0):
+            raise NrwError(f"VoxelRenderer: voxel_size = {voxel_size} (need finite, > 0)")
+        bbx_min, bbx_max = scene_bbox(scene_config, in_sfm=False)
+        scale = float(np.max(bbx_max - bbx_min)) / 2
+        if not (np.isfinite(scale) and scale > 0):
+            raise NrwError(f"VoxelRenderer: the scene's eval_bbx gives scale {scale} (need finite, > 0)")
+        level = int(np.floor(np.log2(2 * scale / voxel_size)))       # gen_octree's rule
+        if not 1 <= level <= 16:
+            raise NrwError(f"VoxelRenderer: voxel_size {voxel_size} in a cube of half-size {scale} gives octree level "
+                           f"{level} (need 1 .. 16)")
+        self.tree, origin, self.scale, self.level = gen_octree(scene_config, self.points, voxel_size, device=self.dev,
+                                                               expand=0, in_sfm=False)
+        self.origin = np.asarray(origin, np.float64)
+        pyr = self.tree["pyramid"].to(torch.int32).contiguous()
+        self.n_leaf = int(pyr[0, self.level])
+        if self.n_leaf == 0:
+            raise NrwError("VoxelRenderer: no source point lies inside the scene's cube (eval_bbx)")
+        self._pyr = (C.c_int * pyr.numel())(*pyr.reshape(-1).tolist())
+        self._origin = (C.c_float * 3)(*self.origin.tolist())
+        self.visible = torch.zeros(self.n_leaf, dtype=torch.uint8, device=self.dev)
+        self.n_hit = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self.status = torch.zeros(1, dtype=torch.int32, device=self.dev)
+
+    def cast(self, height, width, intrinsic, world_to_cam, depth=None, leaf=None):
+        """one view into the given outputs (each may be None); marks `visible` and counts hit pixels in `n_hit`"""
+        L = _lib.lib()
+        E = np.asarray(world_to_cam, np.float64)
+        if E.shape == (3, 4):
+            E = np.concatenate([E, [[0.0, 0.0, 0.0, 1.0]]])
+        c2w = np.linalg.inv(E)
+        fx, fy, cx, cy = _pinhole(intrinsic)
+        with torch.cuda.device(self.dev):
+            check(L.nrw_voxel_cast(ptr(self.tree["octree"]), ptr(self.tree["prefix"]), self._pyr, self.level, self._origin,
+                                   self.scale, _host12(c2w, "VoxelRenderer"), fx, fy, cx, cy, int(height), int(width),
+                                   ptr(self.visible), ptr(depth), ptr(leaf), ptr(self.n_hit), stream_ptr()),
+                  "nrw_voxel_cast")
+
+    def __call__(self, height, width, intrinsic, world_to_cam):
+        height, width = int(height), int(width)
+        if height < 1 or width < 1:
+            raise NrwError(f"VoxelRenderer: image {height} x {width}")
+        depth = torch.empty(height, width, dtype=torch.float32, device=self.dev)
+        leaf = torch.empty(height, width, dtype=torch.int32, device=self.dev)
+        self.cast(height, width, intrinsic, world_to_cam, depth, leaf)
+        return depth, leaf
+
+    def point_leaves(self):
+        """each input point's leaf index (int32 CUDA tensor), -1 outside the open cube; points normalised by the
+        expression of gen_octree"""
+        L = _lib.lib()
+        pn = ((self.points - torch.as_tensor(self.origin, device=self.dev)) / self.scale).contiguous()
+        leaf = torch.empty(pn.shape[0], dtype=torch.int32, device=self.dev)
+        with torch.cuda.device(self.dev):
+            check(L.nrw_voxel_lookup(ptr(self.tree["octree"]), ptr(self.tree["prefix"]), self._pyr, self.level, ptr(pn),
+                                     pn.shape[0], ptr(leaf), ptr(self.status), stream_ptr()), "nrw_voxel_lookup")
+        return leaf
+
+
+def reproj_filter_points(points, scene_config, intrinsics, extrinsics, whs, voxel_size=0.01, device=0):
+    """The visibility mask (numpy bool [n_points]) of a point cloud: True where the point's leaf voxel (octree of the
+    points themselves, gen_octree with expand 0 in their own frame) is the first leaf hit by some pixel's ray of some
+    view.  extrinsics [N,4,4] map the frame of `points` to each camera, intrinsics [N,3,3], whs [N] (width, height).
+    Reads back once, at the end.  Raises NrwError when no view hits any voxel."""
+    r = VoxelRenderer(points, scene_config, voxel_size, device=device)
+    for K, E, (width, height) in zip(intrinsics, extrinsics, whs):
+        r.cast(int(height), int(width), K, E)
+    leaf = r.point_leaves().long()
+    keep = (leaf >= 0) & (r.visible[leaf.clamp(min=0)] != 0)
+    host = torch.cat([r.n_hit, r.status.long(), keep.long()]).cpu().numpy()
+    if host[1]:
+        raise NrwError("reproj_filter_points: a source point's cell is not a leaf of its own octree")
+    if host[0] == 0:
+        raise NrwError("reproj_filter_points: no view hits any voxel of the source points")
+    return host[2:].astype(bool)
+
+
+def _scene_config(data_path):
     import yaml
 
     with open(os.path.join(data_path, "config.yaml"), "r") as fh:
-        scene_config = yaml.load(fh, Loader=yaml.FullLoader)
-    return np.array(scene_config["sfm2gt"])
+        return yaml.load(fh, Loader=yaml.FullLoader)
+
+
+def _sfm2gt(data_path):
+    return np.array(_scene_config(data_path)["sfm2gt"])
 
 
 def _to_gt(pts, sfm_to_gt):
@@ -234,6 +333,8 @@ def get_opts(argv=None):
     parser.add_argument('--voxel_size', type=float, default=0.01, help='voxel size in world coordinate system')
     parser.add_argument('--n_cpus', type=int, default=1, help='accepted and ignored (one process)')
     parser.add_argument('--n_gpus', type=int, default=4, help='accepted and ignored (every view on one device)')
+    parser.add_argument('--point_source', default=False, action="store_true",
+                        help='the source is a point cloud: filter it through its voxel octree (faces are ignored)')
     return parser.parse_args(argv)
 
 
@@ -256,19 +357,25 @@ def main(argv=None):
     extrinsics = get_entrinsics(imdata, img_ids) @ np.linalg.inv(sfm_to_gt)
 
     src = read_ply(args.src_file)
-    if src["faces"].shape[0] == 0:
-        raise NrwError(f"{args.src_file} has no faces: point-cloud sources are not supported")
+    if src["faces"].shape[0] == 0 and not args.point_source:
+        raise NrwError(f"{args.src_file} has no faces: point-cloud sources need --point_source")
     verts = np.asarray(src["vertices"], np.float64)
     tgt = read_ply(args.target_file)
     points = np.asarray(tgt["vertices"], np.float64)
     colors = np.zeros_like(points) if tgt["colors"] is None else tgt["colors"].astype(np.float64) / 255.0
+    if args.point_source and points.shape[0] != verts.shape[0]:
+        raise NrwError(f"--point_source: the target has {points.shape[0]} points and the source {verts.shape[0]}; the "
+                       "kept source indices select target points, so the counts must be equal")
     if not args.gt:
         verts, points = _to_gt(verts, sfm_to_gt), _to_gt(points, sfm_to_gt)
     if not np.isfinite(verts).all():
         raise NrwError(f"{args.src_file}: vertices are not all finite")
 
-    mask = reproj_filter(verts, src["faces"], points, [intrinsics[k] for k in img_ids], extrinsics, [whs[k] for k in img_ids],
-                         voxel_size=args.voxel_size)
+    Ks, Ws = [intrinsics[k] for k in img_ids], [whs[k] for k in img_ids]
+    if args.point_source:
+        mask = reproj_filter_points(verts, _scene_config(args.data_path), Ks, extrinsics, Ws, voxel_size=args.voxel_size)
+    else:
+        mask = reproj_filter(verts, src["faces"], points, Ks, extrinsics, Ws, voxel_size=args.voxel_size)
     rows = np.unique(np.hstack([points[mask], colors[mask]]), axis=0)
     out = os.path.join(args.output_path, "reprojected.ply")
     write_ply(out, rows[:, :3], colors=np.round(rows[:, 3:] * 255.0).astype(np.uint8), double=True)
