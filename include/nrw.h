@@ -386,6 +386,21 @@ NRW_API int nrw_voxel_cast(const uint8_t* octree, const int32_t* prefix, const i
 NRW_API int nrw_voxel_lookup(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid_host, int level,
                              const double* points, long long n_points, int32_t* leaf, int32_t* status, void* stream);
 
+/* ---- training-view selection of the scene split (tools/prepare_data/dataset_filter_utils.py; rules in csrc/viewsel.cu) --
+ * nrw_view_roi_count counts, for every view of one launch, the pixels whose ray passes through the scene sphere
+ * (view_selection's ROI test): views f32 [n_views, 16] = fx, fy, cx, cy, c2w[12] (fp32 [3,4] row-major, columns 1:2
+ * negated as read_meta makes them), hw int32 [n_views, 2] = height, width, both on the device; scene_origin (host f32[3])
+ * and radius (finite, > 0) in fp32.  counts (device int64 [n_views]) is overwritten; a view with height or width < 1, or
+ * height * width > max_hw (1 .. INT32_MAX, the caller's largest view), gets -1.  Rays follow the ray-cache pass's fp32
+ * rule.
+ * nrw_label_static_count adds to count (device int64, not cleared) the number of labels f32 [n] that equal none of the
+ * n_ids <= 8 ids (host int32, each 0 .. 2^24 - 1).  Every host argument is checked before any launch; nothing is read
+ * back to the host. */
+NRW_API int nrw_view_roi_count(const float* views, const int32_t* hw, int n_views, long long max_hw, const float scene_origin[3],
+                               float radius, int64_t* counts, void* stream);
+NRW_API int nrw_label_static_count(const float* labels, long long n, const int32_t* ids_host, int n_ids, int64_t* count,
+                                   void* stream);
+
 /* ---- unit-test hooks ---------------------------------------------------------------------- */
 /* D[M,N] = (sum planes of A)[M,K] * (sum planes of B)[N,K]^T from fp32 inputs: splits into planes in
  * scratch (caller-provided, nrw_gemm_test_scratch_bytes) and runs the selected backend. */

@@ -421,6 +421,18 @@ int nrw_voxel_lookup(const uint8_t* octree, const int32_t* prefix, const int32_t
   NRW_GUARD_END
 }
 
+int nrw_view_roi_count(const float* views, const int32_t* hw, int n_views, long long max_hw, const float scene_origin[3],
+                       float radius, int64_t* counts, void* stream) {
+  NRW_GUARD_BEGIN
+  return view_roi_count(views, hw, n_views, max_hw, scene_origin, radius, counts, S(stream));
+  NRW_GUARD_END
+}
+int nrw_label_static_count(const float* labels, long long n, const int32_t* ids_host, int n_ids, int64_t* count, void* stream) {
+  NRW_GUARD_BEGIN
+  return label_static_count(labels, n, ids_host, n_ids, count, S(stream));
+  NRW_GUARD_END
+}
+
 long long nrw_gemm_test_scratch_bytes(int M, int N, int K) {
   const long long a = round_up((long long)M * K, 512), b = round_up((long long)N * K, 512);
   return (a + b) * 3 * 2 + 4096;

@@ -102,3 +102,10 @@ long long depth_range_scratch_bytes(long long n_points, int n_images);
 int depth_range(const double* xyz, long long n_points, const double* w2c, int n_images, double q_lo, double q_hi, double* out,
                 int64_t* n_front, int32_t* status, void* scratch, cudaStream_t s);
 }  // namespace nrw
+
+// training-view selection of the scene split: ROI pixel counts of many views, static pixels of a semantic map (viewsel.cu)
+namespace nrw {
+int view_roi_count(const float* views, const int32_t* hw, int n_views, long long max_hw, const float origin[3], float radius,
+                   int64_t* counts, cudaStream_t s);
+int label_static_count(const float* labels, long long n, const int32_t* ids, int n_ids, int64_t* count, cudaStream_t s);
+}  // namespace nrw

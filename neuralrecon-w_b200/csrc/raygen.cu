@@ -3,11 +3,11 @@
 // and the per-image near/far percentiles of the SfM points.
 //
 // Per-image pass (pixel p = r*W + c, raster order; cache row o3, d3, near, far, ts, [label,] depth, weight)
-//  * Ray.  i = (float)c, j = (float)r exactly; dx = (i - cx) / fx, dy = (j - cy) / fy, camera direction (dx, -dy, -1).
-//    World direction d_k = (dx*M[k][0] + (-dy)*M[k][1]) + (-M[k][2]) with M = c2w[:, :3] (fp32, row-major),
-//    |d| = sqrt((d_0*d_0 + d_1*d_1) + d_2*d_2), stored d_k / |d|; origin c2w[:, 3].  Every step is one fp32 _rn
-//    operation, no contraction.  c2w is the fp32 rounding of inv(w2c) computed on the host in fp64 with columns 1:2 negated
-//    (read_meta).
+//  * Ray: pixel_ray of pixel_ray.cuh.  i = (float)c, j = (float)r exactly; dx = (i - cx) / fx, dy = (j - cy) / fy, camera
+//    direction (dx, -dy, -1).  World direction d_k = (dx*M[k][0] + (-dy)*M[k][1]) + (-M[k][2]) with M = c2w[:, :3] (fp32,
+//    row-major), |d| = sqrt((d_0*d_0 + d_1*d_1) + d_2*d_2), stored d_k / |d|; origin c2w[:, 3].  Every step is one fp32
+//    _rn operation, no contraction.  c2w is the fp32 rounding of inv(w2c) computed on the host in fp64 with columns 1:2
+//    negated (read_meta).
 //  * RGB = (float)u8 / 255 in fp32 (torchvision ToTensor); decoding and resizing stay on the host (PIL).
 //  * Label (optional) = the semantic map (fp32, sem_h x sem_w) read by cv2's INTER_NEAREST rule for the W x H target:
 //    sx = min(floor(c * (1 / (W / sem_w))), sem_w - 1), sy likewise, in fp64 (OpenCV resizeNN).
@@ -42,6 +42,7 @@
 // status bit 0 = an image with no point in front (its bounds are 0).
 #include "nnsearch.cuh"
 #include "octree_trace.cuh"
+#include "pixel_ray.cuh"
 
 namespace nrw {
 
@@ -113,17 +114,8 @@ __global__ void __launch_bounds__(RG_B) rg_pixel_kernel(RgArgs a, const uint8_t*
   int packed = 0;
   if (p < HW) {
     const int r = p / a.W, c = p - r * a.W;
-    const float dx = NRW_DIV(NRW_SUB((float)c, a.cx), a.fx);
-    const float ndy = -NRW_DIV(NRW_SUB((float)r, a.cy), a.fy);
     float d[3], o[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      d[k] = NRW_ADD(NRW_ADD(NRW_MUL(dx, a.c2w[4 * k]), NRW_MUL(ndy, a.c2w[4 * k + 1])), -a.c2w[4 * k + 2]);
-      o[k] = a.c2w[4 * k + 3];
-    }
-    const float nrm = NRW_SQRT(NRW_ADD(NRW_ADD(NRW_MUL(d[0], d[0]), NRW_MUL(d[1], d[1])), NRW_MUL(d[2], d[2])));
-#pragma unroll
-    for (int k = 0; k < 3; ++k) d[k] = NRW_DIV(d[k], nrm);
+    const float nrm = pixel_ray(a.c2w, a.fx, a.fy, a.cx, a.cy, r, c, o, d);
     bool keep = true;
     float near = a.near_c, far = a.far_c;
     if (a.use_voxel) {

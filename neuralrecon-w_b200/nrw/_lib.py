@@ -144,6 +144,8 @@ def lib():
     L.nrw_voxel_cast.argtypes = [vp, vp, C.POINTER(i32), i32, C.POINTER(f32), f32, C.POINTER(f64), f32, f32, f32, f32, i32, i32,
                                  vp, vp, vp, vp, vp]
     L.nrw_voxel_lookup.argtypes = [vp, vp, C.POINTER(i32), i32, vp, ll, vp, vp, vp]
+    L.nrw_view_roi_count.argtypes = [vp, vp, i32, ll, C.POINTER(f32), f32, vp, vp]
+    L.nrw_label_static_count.argtypes = [vp, ll, C.POINTER(i32), i32, vp, vp]
     L.nrw_gemm_test_scratch_bytes.restype = ll
     L.nrw_gemm_test_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_gemm_test.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp]
@@ -167,7 +169,8 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_nn_index_bytes", "nrw_nn_build", "nrw_nn_query_scratch_bytes", "nrw_nn_query", "nrw_mesh_sample_scratch_bytes",
            "nrw_mesh_sample", "nrw_raster_scratch_bytes", "nrw_raster_depth", "nrw_reproject_scratch_bytes",
            "nrw_reproject_mark", "nrw_raygen_capacity", "nrw_raygen_scratch_bytes", "nrw_raygen_image",
-           "nrw_depth_range_scratch_bytes", "nrw_depth_range", "nrw_voxel_cast", "nrw_voxel_lookup"]
+           "nrw_depth_range_scratch_bytes", "nrw_depth_range", "nrw_voxel_cast", "nrw_voxel_lookup",
+           "nrw_view_roi_count", "nrw_label_static_count"]
 
 
 def check(status, what=""):

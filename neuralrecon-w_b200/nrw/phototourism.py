@@ -80,6 +80,20 @@ def intrinsics(cam, img_downscale):
     return K
 
 
+def camera_poses(images, who):
+    """read_meta step 3: (w2c f64 [n, 4, 4], c2w f64 [n, 3, 4]) of COLMAP images, c2w = inv(w2c)[:, :3] in fp64 with
+    columns 1:2 negated ("right down front" -> "right up back"); the kernels take its fp32 rounding."""
+    bottom = np.array([0, 0, 0, 1.0]).reshape(1, 4)
+    w2c = np.stack([np.concatenate([np.concatenate([im.qvec2rotmat(), im.tvec.reshape(3, 1)], 1), bottom], 0) for im in images], 0)
+    if not np.isfinite(w2c).all():
+        raise NrwError(f"{who}: non-finite camera pose in images.bin")
+    poses = np.linalg.inv(w2c)[:, :3]
+    poses[..., 1:3] *= -1
+    if not np.isfinite(poses).all():
+        raise NrwError(f"{who}: singular camera pose in images.bin")
+    return w2c, poses
+
+
 Scene = collections.namedtuple("Scene", ["root_dir", "sfm_path", "img_downscale", "img_ids", "image_paths", "splits", "Ks",
                                          "w2c", "poses", "imdata", "xyz_world", "table_xyz", "table_err", "config"])
 
@@ -108,15 +122,7 @@ def read_scene(root_dir, img_downscale=1, sfm_path="sparse"):
     if not img_ids:
         raise NrwError("read_scene: no tsv image is in images.bin")
     Ks = {id_: intrinsics(cams[imdata[id_][0].camera_id], img_downscale) for id_ in img_ids}
-    bottom = np.array([0, 0, 0, 1.0]).reshape(1, 4)
-    w2c = np.stack([np.concatenate([np.concatenate([imdata[i][0].qvec2rotmat(), imdata[i][0].tvec.reshape(3, 1)], 1), bottom], 0)
-                    for i in img_ids], 0)
-    if not np.isfinite(w2c).all():
-        raise NrwError("read_scene: non-finite camera pose in images.bin")
-    poses = np.linalg.inv(w2c)[:, :3]
-    poses[..., 1:3] *= -1
-    if not np.isfinite(poses).all():
-        raise NrwError("read_scene: singular camera pose in images.bin")
+    w2c, poses = camera_poses([imdata[i][0] for i in img_ids], "read_scene")
     pts = colmap.read_points3d(os.path.join(base, "points3D.bin"))
     n_table = int(pts["id"].max()) + 1 if len(pts["id"]) else 1
     table_xyz = np.ones((n_table, 3), np.float64)      # ids absent from points3D.bin read as the reference's ones

@@ -14,7 +14,7 @@ from ._lib import NrwError, check, ptr, stream_ptr
 from .engine import Engine, make_render_cfg, make_sampler_cfg
 
 # ADE20K ids of the labels the path uses (datasets/mask_utils.py:11-160)
-LABEL_IDS = {"sky": 2, "road": 6, "person": 12, "car": 20, "minibike": 116, "bicycle": 127}
+LABEL_IDS = {"sky": 2, "tree": 4, "road": 6, "person": 12, "car": 20, "minibike": 116, "bicycle": 127}
 
 
 class NeuconWRenderer:
