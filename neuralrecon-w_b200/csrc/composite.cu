@@ -373,13 +373,15 @@ int composite_forward(const nrw_render_cfg& cfg, const nrw_render_io& io, const 
   NRW_CHECK(T <= 1280, NRW_ERR_ARG, "composite: T=%d samples per ray exceeds 1280", T);
   NRW_CUDA_OK(cudaMemsetAsync(ge_acc, 0, 2 * sizeof(float), s));
   const int grid = cdiv((long long)cfg.R * 32, 128);
-  switch (pick_cpl(T)) {
-    case 5: composite_fwd_kernel<5><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc); break;
-    case 8: composite_fwd_kernel<8><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc); break;
-    case 16: composite_fwd_kernel<16><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc); break;
-    default: composite_fwd_kernel<40><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc);
+  if (grid > 0) {  // R = 0: no per-ray work, but gradient_error / sv_relax_sum are still finalised (to 0)
+    switch (pick_cpl(T)) {
+      case 5: composite_fwd_kernel<5><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc); break;
+      case 8: composite_fwd_kernel<8><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc); break;
+      case 16: composite_fwd_kernel<16><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc); break;
+      default: composite_fwd_kernel<40><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, rgb, bg_alpha, bg_rgb, ge_acc);
+    }
+    NRW_LAUNCH_OK();
   }
-  NRW_LAUNCH_OK();
   ge_finalize_kernel<<<1, 1, 0, s>>>(ge_acc, io.gradient_error, io.sv_relax_sum);
   NRW_LAUNCH_OK();
   return NRW_OK;
@@ -393,6 +395,7 @@ int composite_backward(const nrw_render_cfg& cfg, const nrw_render_io& io, const
   NRW_CHECK(T <= 1280, NRW_ERR_ARG, "composite: T=%d samples per ray exceeds 1280", T);
   if (d_inv_s) NRW_CUDA_OK(cudaMemsetAsync(d_inv_s, 0, sizeof(float), s));
   const int grid = cdiv((long long)cfg.R * 32, 128);
+  if (grid == 0) return NRW_OK;  // R = 0: nothing to launch; grad_inv_s stays zeroed
 #define NRW_BWD(C) composite_bwd_kernel<C><<<grid, 128, 0, s>>>(cfg, io, g, sdf, nrm, rgb, bg_alpha, bg_rgb, d_sdf, d_nrm, d_rgb, d_bga, d_bgc, d_inv_s)
   switch (pick_cpl(T)) {
     case 5: NRW_BWD(5); break;
