@@ -173,11 +173,15 @@ static int mm_dw(nrw_ctx& c, Planes dY, Planes X, int M, int layer, cudaStream_t
   GemmDesc g;
   g.A = dY; g.B = X; g.n_planes = c.cur_planes;
   g.M = L.Np; g.N = L.Kp; g.K = M; g.mn_major = 1;
-  const int tiles = cdiv(g.M, 128) * cdiv(g.N, gemm_tc_tile_n(g.N));
+  Epi e;
+  e.out_f32 = c.dW(layer); e.ld_f32 = L.Kp; e.atomic = 1;
+  g.epi = e;
+  const int tiles = cdiv(g.M, gemm_tc_tile_m(g)) * cdiv(g.N, gemm_tc_tile_n(g.N));
   int dev = 0, n_sm = 0;
   NRW_CUDA_OK(cudaGetDevice(&dev));
   NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-  int ks = 2 * n_sm / tiles;   // about two work items per SM
+  // at most two full waves of work items (512 x 512 on 132 SMs: 8 tiles x 33 slices = 264 items)
+  int ks = 2 * n_sm / tiles;
   const int max_ks = M / 512 > 0 ? M / 512 : 1;
   if (ks > max_ks) ks = max_ks;
   if (ks < 1) ks = 1;
@@ -186,9 +190,6 @@ static int mm_dw(nrw_ctx& c, Planes dY, Planes X, int M, int layer, cudaStream_t
   const int kb_per = cdiv(kb_total, ks);
   ks = cdiv(kb_total, kb_per);
   g.k_slices = ks;
-  Epi e;
-  e.out_f32 = c.dW(layer); e.ld_f32 = L.Kp; e.atomic = 1;
-  g.epi = e;
   return gemm(c.backend, g, s);
 }
 static int bias_grad(nrw_ctx& c, Planes dY, int M, int layer, cudaStream_t s) {

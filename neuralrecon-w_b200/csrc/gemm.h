@@ -43,6 +43,14 @@ int sdf_fused_forward(const SdfFusedDesc& d, cudaStream_t stream);
 long long gemm_tc_launch_count();
 // output columns of one gemm_tc tile (the caller of a split-K GEMM sizes k_slices from the tile count)
 inline int gemm_tc_tile_n(int N) { return N <= 64 ? 64 : 128; }
+// One-plane weight gradients (MN-major, out_f32 += scale * A^T B and nothing else) with M >= 256 and N > 64 run 256 x 128
+// items that both consumer warpgroups share; every other GEMM runs 128-row items.
+inline bool gemm_tc_dw_coop(const GemmDesc& g) {
+  const Epi& e = g.epi;
+  return g.mn_major && g.n_planes == 1 && g.M >= 256 && g.N > 64 && e.atomic && e.out_f32 && e.ld_f32 % 2 == 0 &&
+         (reinterpret_cast<uintptr_t>(e.out_f32) & 7) == 0 && !e.bias && !e.rowvec && !e.out_pre && !e.colsum;
+}
+inline int gemm_tc_tile_m(const GemmDesc& g) { return gemm_tc_dw_coop(g) ? 256 : 128; }
 // debug: when non-null, every tensor-core GEMM launch accumulates per-CTA cycle attribution into buf[SMs*16]
 void gemm_tc_set_profile_buffer(unsigned long long* buf);
 // measurement: CUDA events around every tensor-core GEMM launch (on the launching stream)

@@ -20,6 +20,12 @@
 // * mn_major=1 consumes both operands "transposed" straight from their natural row-major
 //   [rows=K][cols=M|N] layout (MN-major wgmma descriptors) - used for weight gradients
 //   dW = dY^T X with split-K over the sample dimension and fp32 atomics in the epilogue.
+// * MN_COOP (one-plane weight gradients with M >= 256, gemm_tc_dw_coop): a work item is a 256 x 128 tile x K-slice that
+//   both consumer warpgroups run at the same time, warpgroup wg on rows 128 wg .. +127 (two m64n128 halves), both reading
+//   the stage's one B tile.  Per 64-row k-block that moves 48 KB for 4.2 MFLOP instead of 32 KB for 2.1 MFLOP.  No turn
+//   barrier: each stage's empty barrier counts all 8 consumer warps.  The epilogue is one fp32 vector reduction
+//   (red.global.add.v2.f32) per accumulator pair straight from the fragment: no staging tile and no named barriers, while
+//   the producer already loads the next item's k-blocks.
 #include <stdlib.h>
 
 #include <mutex>
@@ -44,6 +50,7 @@ static constexpr int EPI_COLS = 64;                    // columns per epilogue r
 static constexpr int EPI_WG_BYTES = 64 * EPI_COLS * 4; // one warpgroup's staging tile [64 rows][64 columns]
 static constexpr int CS_BYTES = 1024;                  // column-sum accumulators: 128 columns of the current n-tile per warpgroup
 static constexpr int BAR_TURN = 4;                     // named barriers 4 + wg: warpgroup wg's turn at the tensor cores
+static constexpr int MN_COOP = 2;                      // MN_MAJOR value of the cooperative 256-row weight-gradient schedule
 static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 32 * N_CONSUMER_WARPS <= 65536, "register file");
 static constexpr int BAR_BYTES = 256;                  // 2 x MAX_STAGES mbarriers
 static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + 2 * EPI_WG_BYTES + CS_BYTES;
@@ -66,7 +73,7 @@ struct TcParams {
   // optional cycle attribution (debug): per CTA 16 counters
   //  [0] producer: waiting for a free stage   [5] kernel cycles
   //  first warp of consumer warpgroup wg, o = 8 wg: [1 + o] waiting for TMA data   [3 + o] waiting for its turn at the
-  //  tensor cores   [4 + o] epilogue   [6 + o] tiles
+  //  tensor cores   [4 + o] epilogue   [6 + o] tiles (MN_COOP: both warpgroups count every non-empty item)
   unsigned long long* prof;
 };
 #define NRW_PROF_T0(cond) const long long _t0 = (cond) ? clock64() : 0
@@ -130,6 +137,10 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 // generic-proxy shared-memory stores -> visible to the tensor core's (async proxy) reads
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// out[0], out[1] += a, b: one sm_90 vector fp32 reduction (out 8-byte aligned)
+__device__ __forceinline__ void red_add_v2(float* out, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(out), "f"(a), "f"(b) : "memory");
+}
 
 // wgmma matrix descriptor (sm_90), 128B swizzle:
 //   bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 1 (128B swizzle)
@@ -208,11 +219,15 @@ NRW_WGMMA_N128(1, 1)
 //   n_planes==1: (0,0); ==2: (0,1),(1,0),(0,0); ==3: (0,2),(2,0),(1,1),(0,1),(1,0),(0,0)
 // With q = n_products-1-p (q=0 is (hi,hi)): a_plane = nibble q of 0x021010, b_plane = nibble q of 0x201100.
 
-// EK: compile-time epilogue kind (epilogue_fast.cuh); MN-major launches use EK_GENERIC.
+// EK: compile-time epilogue kind (epilogue_fast.cuh); MN-major launches use EK_GENERIC.  MN_MAJOR: 0 K-major, 1 MN-major
+// ping-pong, MN_COOP MN-major with 256-row items shared by both warpgroups.
 template <int BN, int MN_MAJOR, int EK>
 __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
   static_assert(BN == 64 || BN == 128, "wgmma tile width");
-  constexpr int A_TILE = BM * BK * 2;
+  constexpr bool COOP = MN_MAJOR == MN_COOP;
+  static_assert(!COOP || (BN == 128 && EK == EK_GENERIC), "the cooperative schedule is the 256 x 128 weight-gradient tile");
+  constexpr int TM = COOP ? 2 * BM : BM;        // rows of a work item
+  constexpr int A_TILE = TM * BK * 2;
   constexpr int B_TILE = BN * BK * 2;
   constexpr int WG_A = 64 * BK * 2;           // one 64-row half of the A tile (K-major: 64 rows; MN-major: one 64-wide slab)
   extern __shared__ uint8_t smem_raw[];
@@ -237,7 +252,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     }
     for (int i = 0; i < MAX_STAGES; ++i) {
       mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, 4);              // the four warps of the stage's consuming warpgroup
+      mbar_init(bar_empty + 8 * i, COOP ? 8 : 4);   // the four warps of the stage's consuming warpgroup (COOP: both)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -260,7 +275,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
         const int ks = item % p.k_slices;
         const int t = item / p.k_slices;
-        const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * BM;
+        const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * TM;
         const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
         for (int kb = kb0; kb < kb1; ++kb) {
           {
@@ -277,7 +292,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
               tma_load_2d(sb + pl * B_TILE, &p.tmB[pl], bar_full + 8 * s, kb * BK, n0);
             } else {
 #pragma unroll
-              for (int sl = 0; sl < BM / 64; ++sl)
+              for (int sl = 0; sl < TM / 64; ++sl)
                 tma_load_2d(sa + pl * A_TILE + sl * (64 * BK * 2), &p.tmA[pl], bar_full + 8 * s,
                             m0 + 64 * sl, kb * BK);
 #pragma unroll
@@ -289,6 +304,88 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
           if (++s == stages) { s = 0; ph ^= 1; }
         }
       }
+    }
+  } else if constexpr (COOP) {
+    // ===================== consumers: both warpgroups on every item, warpgroup wg on rows 128 wg .. +127 =====================
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = warp >> 2, wi = warp & 3;
+    const uint32_t smem0 = smem_u32(smem);
+    const uint64_t desc_hi = make_gdesc(0, 64 * BK * 2, 1024);   // MN-major: LBO = stride between 64-wide slabs, SBO = 8 k-rows
+    constexpr uint32_t KSTEP = 16 * 128;                          // bytes per wgmma K=16
+    const bool prof = p.prof != nullptr && wi == 0 && lane == 0;
+    const int po = 8 * wg;
+    const int n_lim = min(p.N, p.epi.n_store);
+    int s = 0;
+    uint32_t ph = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int ks = item % p.k_slices;
+      const int t = item / p.k_slices;
+      const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * TM;
+      const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
+      float acc[2][BN / 2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.0f;
+      int prev_s = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        {
+          NRW_PROF_T0(prof);
+          mbar_wait(bar_full + 8 * s, ph);
+          NRW_PROF_ADD(prof, 1 + po);
+        }
+        const uint32_t sa = smem0 + s * stage_bytes;
+        const uint32_t sb = smem0 + s * stage_bytes + P * A_TILE;
+        wgmma_fence();
+        for (int pr = 0; pr < n_prod; ++pr) {
+          const int q = 4 * (n_prod - 1 - pr);
+          const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
+          const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE + 2 * wg * WG_A) & 0x3FFFFu) >> 4);
+          const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)                  // 64-wide A slab 2 wg + h
+              wgmma_bf16<BN, 1, 1>(acc[h], da + ((h * WG_A + k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
+        }
+        wgmma_commit();
+        acc_fence(acc[0]);
+        acc_fence(acc[1]);
+        if (prev_s >= 0) {                                // the previous stage's MMAs have completed: hand it back
+          wgmma_wait<1>();
+          acc_fence(acc[0]);
+          acc_fence(acc[1]);
+          if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+        }
+        prev_s = s;
+        if (++s == stages) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      acc_fence(acc[0]);
+      acc_fence(acc[1]);
+      if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+      if (kb1 <= kb0) continue;                           // an empty K-slice stores nothing
+      NRW_PROF_T0(prof);
+      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6 + po], 1ull);
+      // fragment of warp wi in half h: acc[h][4j + {0,1}] = row 128 wg + 64 h + 16 wi + lane / 4, columns 8 j + 2 (lane % 4)
+      // + {0,1}; acc[h][4j + {2,3}] = the same columns of row + 8
+      const int c0 = n0 + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r8 = 0; r8 < 2; ++r8) {
+          const int row = m0 + 128 * wg + 64 * h + 16 * wi + (lane >> 2) + 8 * r8;
+          if (row >= p.M) continue;
+          float* dst = p.epi.out_f32 + (long long)row * p.epi.ld_f32;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int c = c0 + 8 * j;
+            const float x0 = acc[h][4 * j + 2 * r8] * p.epi.scale, x1 = acc[h][4 * j + 2 * r8 + 1] * p.epi.scale;
+            if (c + 1 < n_lim) red_add_v2(dst + c, x0, x1);
+            else if (c < n_lim) atomicAdd(dst + c, x0);
+          }
+        }
+      NRW_PROF_ADD(prof, 4 + po);
     }
   } else {
     // ===================== consumers: ping-pong warpgroups, each the MMAs and then the epilogue of its own items =====================
@@ -626,11 +723,12 @@ static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
   if (!n_sm_dev[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm_dev[dev], cudaDevAttrMultiProcessorCount, dev));
   const int n_sm = n_sm_dev[dev];
   // 128 x 128 tiles (one warpgroup, two m64n128 halves): with two operand planes that is 64 KB per k-block and 3 TMA stages
-  const int BN = g.N <= 64 ? 64 : 128;
+  const int BN = gemm_tc_tile_n(g.N);
+  const bool coop = gemm_tc_dw_coop(g);
   TcParams p;
   memset(&p, 0, sizeof(p));
   p.M = g.M; p.N = g.N; p.K = g.K; p.n_planes = g.n_planes; p.k_slices = g.k_slices;
-  p.m_tiles = cdiv(g.M, BM); p.n_tiles = cdiv(g.N, BN);
+  p.m_tiles = cdiv(g.M, gemm_tc_tile_m(g)); p.n_tiles = cdiv(g.N, BN);
   p.epi = g.epi;
   p.prof = g_prof_ptr;
   for (int pl = 0; pl < g.n_planes; ++pl) {
@@ -646,6 +744,7 @@ static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
   const int ek = g.mn_major ? EK_GENERIC : pick_epi_kind(g.epi);
   NRW_CHECK(ek >= 0 && (ek != EK_FWD_HEAD || g.N == 512), NRW_ERR_ARG,
             "gemm_tc: the fused SDF-head epilogue needs N = 512, bias + softplus and no other output");
+  if (coop) return launch<128, MN_COOP, EK_GENERIC>(p, n_sm, dev, stream);
   if (g.mn_major) return BN == 64 ? launch<64, 1, EK_GENERIC>(p, n_sm, dev, stream) : launch<128, 1, EK_GENERIC>(p, n_sm, dev, stream);
   if (BN == 64) return launch<64, 0, EK_GENERIC>(p, n_sm, dev, stream);
   switch (ek) {
