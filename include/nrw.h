@@ -408,6 +408,20 @@ NRW_API long long nrw_gemm_test_scratch_bytes(int M, int N, int K);
 NRW_API int nrw_gemm_test(int backend, int n_planes, int mn_major, int k_slices, int M, int N, int K,
                           const float* A, const float* B, const float* bias, int act, float* D,
                           void* scratch, void* stream);
+/* A backward layer's data GEMM and weight gradient in one paired tensor-core launch (paired = 1; the launch must be eligible,
+ * else NRW_ERR_ARG), or as two launches, weight gradient first (paired = 0).  One-plane bf16 operands:
+ *   data  out[M, N] = epilogue(A[M, K] B[N, K]^T) of kind `kind`, all side streams [M, N] with ld N:
+ *         0 GENERIC   planes out_pl, column sums into colsum (if non-NULL)
+ *         1 TANGENT   gate from the bf16 plane side_h (u / scale), aux_q = side_f (NULL: colvec broadcast), out2 (fp32),
+ *                     planes out_pl, or out_f32 when non-NULL
+ *         2 REVERSE   [+ rowvec (x) colvec], gate from side_h, + side_f, planes out_pl, colsum
+ *         3 RELU_BWD  [+ rowvec (x) colvec], mask by the bf16 side_h > 0, planes out_pl, colsum
+ *         with the output scale `scale` and the column bound n_store;
+ *   dW    dW[Mw, Nw] (fp32) += dY[Kw, Mw]^T X[Kw, Nw], split into k_slices K-slices. */
+NRW_API int nrw_gemm_pair_test(int paired, int kind, int M, int N, int K, int Mw, int Nw, int Kw, int k_slices,
+                               const void* A, const void* B, const void* dY, const void* X, const void* side_h,
+                               const float* side_f, const float* rowvec, const float* colvec, float scale, int n_store,
+                               void* out_pl, float* out_f32, float* out2, float* colsum, float* dW, void* stream);
 NRW_API long long nrw_launch_count(void);
 /* measurement: while enabled, every tensor-core GEMM launch is bracketed by CUDA events on its stream; a call with
  * out5 != NULL synchronises those events and returns {sum of kernel ms, algorithmic FLOP (2MNK), MMA FLOP

@@ -459,6 +459,42 @@ int nrw_gemm_test(int backend, int n_planes, int mn_major, int k_slices, int M, 
   return gemm(backend, g, S(stream));
   NRW_GUARD_END
 }
+int nrw_gemm_pair_test(int paired, int kind, int M, int N, int K, int Mw, int Nw, int Kw, int k_slices, const void* A,
+                       const void* B, const void* dY, const void* X, const void* side_h, const float* side_f,
+                       const float* rowvec, const float* colvec, float scale, int n_store, void* out_pl, float* out_f32,
+                       float* out2, float* colsum, float* dW, void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(kind >= 0 && kind <= 3 && k_slices >= 1 && scale != 0.0f, NRW_ERR_ARG, "gemm_pair_test: kind=%d k_slices=%d", kind,
+            k_slices);
+  auto plane = [](const void* p, long long rows, int ld) { return Planes{reinterpret_cast<bf16*>(const_cast<void*>(p)), rows * ld, ld}; };
+  GemmPair pr;
+  GemmDesc& d = pr.data;
+  d.A = plane(A, M, K); d.B = plane(B, N, K); d.n_planes = 1; d.M = M; d.N = N; d.K = K;
+  Epi& e = d.epi;
+  e.scale = scale; e.n_store = n_store; e.rowvec = rowvec; e.colvec = rowvec ? colvec : nullptr;
+  if (kind == 1 || kind == 2) {   // gates from one bf16 plane of u (x 1/scale: the skip layer's input)
+    e.aux_u = plane(side_h, M, N); e.aux_u_planes = 1; e.aux_u_scale = 1.0f / scale;
+  }
+  if (kind == 1) {
+    e.aux_q = side_f ? side_f32(side_f, N) : side_f32(colvec, 0);
+    e.aux_q_bcast = side_f ? 0 : 1;
+    e.out2 = side_f32(out2, N);
+    e.rowvec = e.colvec = nullptr;
+  }
+  if (kind == 2) e.aux_add = side_f32(side_f, N);
+  if (kind == 3) { e.aux_relu = reinterpret_cast<const bf16*>(side_h); e.ld_relu = N; }
+  if (kind == 1 && out_f32) { e.out_f32 = out_f32; e.ld_f32 = N; }
+  else { e.out_pl = plane(out_pl, M, N); e.n_planes = 1; }
+  if (kind != 1) e.colsum = colsum;
+  GemmDesc& w = pr.dw;
+  w.A = plane(dY, Kw, Mw); w.B = plane(X, Kw, Nw); w.n_planes = 1; w.M = Mw; w.N = Nw; w.K = Kw; w.mn_major = 1;
+  w.k_slices = k_slices;
+  w.epi.out_f32 = dW; w.epi.ld_f32 = Nw; w.epi.atomic = 1;
+  if (paired) return gemm_tc_pair(pr, S(stream));
+  NRW_TRY(gemm_tc(w, S(stream)));
+  return gemm_tc(d, S(stream));
+  NRW_GUARD_END
+}
 long long nrw_launch_count(void) { return g_kernel_launches; }
 int nrw_gemm_timing(int enable, double* out5 /* host: ms, algorithmic FLOP, MMA FLOP, launches, algorithmic HBM bytes; may be NULL */) {
   NRW_GUARD_BEGIN

@@ -160,17 +160,19 @@ int carve_workspace(nrw_ctx& c, void* base, long long bytes, int chunk_rows, int
 // ---------------------------------------------------------------------------------------------
 // GEMM helpers
 // ---------------------------------------------------------------------------------------------
-static int mm(nrw_ctx& c, Planes A, Planes B, int M, int N, int K, Epi e, cudaStream_t s) {
+static GemmDesc mm_desc(nrw_ctx& c, Planes A, Planes B, int M, int N, int K, Epi e) {
   GemmDesc g;
   g.A = A; g.B = B; g.n_planes = c.cur_planes; g.M = M; g.N = N; g.K = K; g.mn_major = 0; g.k_slices = 1;
   if (e.out_pl.p) e.n_planes = c.cur_planes;
   g.epi = e;
-  return gemm(c.backend, g, s);
+  return g;
+}
+static int mm(nrw_ctx& c, Planes A, Planes B, int M, int N, int K, Epi e, cudaStream_t s) {
+  return gemm(c.backend, mm_desc(c, A, B, M, N, K, e), s);
 }
 // dW[layer] += dY^T X   (dY [M, Np], X [M, Kx]); atomically accumulated into the gradient scratch
-static int mm_dw(nrw_ctx& c, Planes dY, Planes X, int M, int layer, cudaStream_t s) {
+static int dw_desc(nrw_ctx& c, Planes dY, Planes X, int M, int layer, GemmDesc& g) {
   const PackedLayer& L = c.pm.layers[layer];
-  GemmDesc g;
   g.A = dY; g.B = X; g.n_planes = c.cur_planes;
   g.M = L.Np; g.N = L.Kp; g.K = M; g.mn_major = 1;
   Epi e;
@@ -190,7 +192,28 @@ static int mm_dw(nrw_ctx& c, Planes dY, Planes X, int M, int layer, cudaStream_t
   const int kb_per = cdiv(kb_total, ks);
   ks = cdiv(kb_total, kb_per);
   g.k_slices = ks;
+  return NRW_OK;
+}
+static int mm_dw(nrw_ctx& c, Planes dY, Planes X, int M, int layer, cudaStream_t s) {
+  GemmDesc g;
+  NRW_TRY(dw_desc(c, dY, X, M, layer, g));
   return gemm(c.backend, g, s);
+}
+// A backward layer: dW[layer] += dY^T X and the data GEMM A B^T -> e, which do not read each other's outputs.  On the
+// tensor-core backend they share one launch when gemm_tc_pair_ok (NRW_BWD_PAIR=0: never); otherwise they run as two
+// launches, dW first.
+static int mm_bwd(nrw_ctx& c, Planes dY, Planes X, int layer, Planes A, Planes B, int M, int N, int K, Epi e,
+                  cudaStream_t s) {
+  static const int pair = getenv("NRW_BWD_PAIR") ? atoi(getenv("NRW_BWD_PAIR")) : 1;
+  GemmPair pr;
+  pr.data = mm_desc(c, A, B, M, N, K, e);
+  NRW_TRY(dw_desc(c, dY, X, M, layer, pr.dw));
+  if (pair && c.backend == NRW_GEMM_TCGEN05 && gemm_tc_pair_ok(pr)) {
+    pr.dw.k_slices = gemm_tc_pair_k_slices(M);
+    return gemm_tc_pair(pr, s);
+  }
+  NRW_TRY(gemm(c.backend, pr.dw, s));
+  return gemm(c.backend, pr.data, s);
 }
 static int bias_grad(nrw_ctx& c, Planes dY, int M, int layer, cudaStream_t s) {
   return launch_colsum(dY, c.cur_planes, nullptr, 0, M, c.pm.layers[layer].Np, nullptr, c.db(layer), nullptr, s);
@@ -344,31 +367,26 @@ int color_chunk_backward(nrw_ctx& c, int M, const float* d_rgb, const float* d_n
   int cur = 0;
   NRW_TRY(bias_grad(c, c.dX[0], M, L_CL0 + 3, s));
   for (int l = 3; l >= 1; --l) {
-    NRW_TRY(mm_dw(c, c.dX[cur], c.X[l], M, L_CL0 + l, s));
     Epi e; e.aux_relu = c.X[l].p; e.ld_relu = 256; e.out_pl = c.dX[1 - cur]; e.colsum = c.db(L_CL0 + l - 1);
-    NRW_TRY(mm(c, c.dX[cur], c.WT(L_CL0 + l), M, 256, 256, e, s));
+    NRW_TRY(mm_bwd(c, c.dX[cur], c.X[l], L_CL0 + l, c.dX[cur], c.WT(L_CL0 + l), M, 256, 256, e, s));
     cur = 1 - cur;
   }
-  NRW_TRY(mm_dw(c, c.dX[cur], c.IN2, M, L_CL0, s));
   { Epi e; e.aux_relu = c.IN2.p; e.ld_relu = 192; e.out_pl = c.dH2; e.colsum = c.db(L_CS1);
-    NRW_TRY(mm(c, c.dX[cur], c.WT(L_CL0), M, 128, 256, e, s)); }
+    NRW_TRY(mm_bwd(c, c.dX[cur], c.IN2, L_CL0, c.dX[cur], c.WT(L_CL0), M, 128, 256, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 64;
     NRW_TRY(mm(c, c.dX[cur], rows(c.WT(L_CL0), 128), M, 64, 256, e, s)); }
   add_normal_grad_kernel<<<cdiv(M, 256), 256, 0, s>>>(c.c_dn, d_nrm_comp, c.tail, M);
   NRW_LAUNCH_OK();
   // static_linear_1: H1 -> IN2[:, :128]
-  NRW_TRY(mm_dw(c, c.dH2, c.H1, M, L_CS1, s));
   { Epi e; e.aux_relu = c.H1.p; e.ld_relu = 128; e.out_pl = c.dH1; e.colsum = c.db(L_CS0);
-    NRW_TRY(mm(c, c.dH2, c.WT(L_CS1), M, 128, 128, e, s)); }
+    NRW_TRY(mm_bwd(c, c.dH2, c.H1, L_CS1, c.dH2, c.WT(L_CS1), M, 128, 128, e, s)); }
   // static_linear_0: IN1 [xf | viewPE | a] -> H1
-  NRW_TRY(mm_dw(c, c.dH1, c.IN1, M, L_CS0, s));
-  { Epi e; e.out_pl = c.dXF; e.colsum = c.db(L_CX); NRW_TRY(mm(c, c.dH1, c.WT(L_CS0), M, 512, 128, e, s)); }
+  { Epi e; e.out_pl = c.dXF; e.colsum = c.db(L_CX); NRW_TRY(mm_bwd(c, c.dH1, c.IN1, L_CS0, c.dH1, c.WT(L_CS0), M, 512, 128, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
     NRW_TRY(mm(c, c.dH1, rows(c.WT(L_CS0), 512), M, 128, 128, e, s)); }
   if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, rows_per_src, d_a_rays, 1, s));
   // xyz_encoding_final: FEAT -> IN1[:, :512]
-  NRW_TRY(mm_dw(c, c.dXF, c.FEAT, M, L_CX, s));
-  { Epi e; e.out_pl = c.DFEAT; e.colsum = c.db(L_SDF8F); NRW_TRY(mm(c, c.dXF, c.WT(L_CX), M, 512, 512, e, s)); }
+  { Epi e; e.out_pl = c.DFEAT; e.colsum = c.db(L_SDF8F); NRW_TRY(mm_bwd(c, c.dXF, c.FEAT, L_CX, c.dXF, c.WT(L_CX), M, 512, 512, e, s)); }
   return NRW_OK;
 }
 
@@ -388,7 +406,6 @@ int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, 
   // tangent sweep: derivative of the gradient chain
   for (int l = 0; l < 8; ++l) {
     Planes DQl = dq_buf(c, l);
-    NRW_TRY(mm_dw(c, c.G[l], DQl, M, L_SDF0 + l, s));
     Epi e;
     gate_from(c, e, l, c.gate_planes());
     if (l == 7) { e.aux_q = side_f32(w0, 0); e.aux_q_bcast = 1; } else { e.aux_q = c.Q[l + 1]; }
@@ -396,11 +413,11 @@ int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, 
     if (l == 3) { e.scale = INV_SQRT2; e.n_store = 473; }
     if (l < 7) e.out_pl = dq_buf(c, l + 1);
     else { e.out_f32 = c.DQ8f; e.ld_f32 = 512; }
-    NRW_TRY(mm(c, DQl, c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
+    // (l = 0: the 512 x 64 weight gradient cannot pair and runs first, on its own)
+    NRW_TRY(mm_bwd(c, c.G[l], DQl, L_SDF0 + l, DQl, c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
   }
   NRW_TRY(launch_colsum(Planes{nullptr, 0, 0}, P, c.DQ8f, 512, M, 512, nullptr, c.gs + H.d_sdf_w0, nullptr, s));
   // reverse sweep
-  NRW_TRY(mm_dw(c, c.DFEAT, c.U[8], M, L_SDF8F, s));   // (db of lin8[1:] was accumulated by the colour backward)
   NRW_TRY(launch_colsum(c.U[8], P, nullptr, 0, M, 512, d_sdf, c.gs + H.d_sdf_w0, c.gs + H.d_sdf_b0, s));
   {
     Epi e;
@@ -409,18 +426,18 @@ int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, 
     e.aux_add = c.DA2[7];
     e.out_pl = c.DA[1];
     e.colsum = c.db(L_SDF0 + 7);
-    NRW_TRY(mm(c, c.DFEAT, c.WT(L_SDF8F), M, 512, 512, e, s));
+    // (db of lin8[1:] was accumulated by the colour backward)
+    NRW_TRY(mm_bwd(c, c.DFEAT, c.U[8], L_SDF8F, c.DFEAT, c.WT(L_SDF8F), M, 512, 512, e, s));
   }
   for (int l = 7; l >= 1; --l) {
     Planes cur = c.DA[l & 1];
-    NRW_TRY(mm_dw(c, cur, c.U[l], M, L_SDF0 + l, s));
     Epi e;
     gate_from(c, e, l - 1, c.gate_planes());
     e.aux_add = c.DA2[l - 1];
     e.out_pl = c.DA[(l - 1) & 1];
     e.colsum = c.db(L_SDF0 + l - 1);
     if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }
-    NRW_TRY(mm(c, cur, c.WT(L_SDF0 + l), M, 512, 512, e, s));
+    NRW_TRY(mm_bwd(c, cur, c.U[l], L_SDF0 + l, cur, c.WT(L_SDF0 + l), M, 512, 512, e, s));
   }
   NRW_TRY(mm_dw(c, c.DA[0], c.U0, M, L_SDF0, s));
   return NRW_OK;
@@ -436,13 +453,12 @@ int nerf_chunk_backward(nrw_ctx& c, int M, const float* d_bga, const float* d_bg
   int cur = 0;
   NRW_TRY(bias_grad(c, c.dNA[0], M, L_NS0 + 3, s));
   for (int l = 3; l >= 1; --l) {
-    NRW_TRY(mm_dw(c, c.dNA[cur], c.AP[l], M, L_NS0 + l, s));
     Epi e; e.aux_relu = c.AP[l].p; e.ld_relu = 128; e.out_pl = c.dNA[1 - cur]; e.colsum = c.db(L_NS0 + l - 1);
-    NRW_TRY(mm(c, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
+    NRW_TRY(mm_bwd(c, c.dNA[cur], c.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
     cur = 1 - cur;
   }
-  NRW_TRY(mm_dw(c, c.dNA[cur], c.FEATN, M, L_NS0, s));
-  { Epi e; e.out_pl = c.dNF; e.colsum = c.db(L_NF); NRW_TRY(mm(c, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
+  { Epi e; e.out_pl = c.dNF; e.colsum = c.db(L_NF);
+    NRW_TRY(mm_bwd(c, c.dNA[cur], c.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
     NRW_TRY(mm(c, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
   if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, T, d_a_rays, 1, s));
@@ -450,16 +466,15 @@ int nerf_chunk_backward(nrw_ctx& c, int M, const float* d_bga, const float* d_bg
   NRW_TRY(launch_head_bwd(1, c.NH[8], P, 256, M, c.f_area + H.na_w, d_bga, c.c_density, c.c_dists, 2,
                           Planes{nullptr, 0, 0}, c.c_ddens, c.gs + H.d_na_w, c.gs + H.d_na_b, s));
   // feature_linear: NH[8] -> FEATN[:, :256]
-  NRW_TRY(mm_dw(c, c.dNF, c.NH[8], M, L_NF, s));
   { Epi e; e.rowvec = c.c_ddens; e.colvec = c.f_area + H.na_w; e.aux_relu = c.NH[8].p; e.ld_relu = 256;
     e.out_pl = c.dNH[0]; e.colsum = c.db(L_N0 + 7);
-    NRW_TRY(mm(c, c.dNF, c.WT(L_NF), M, 256, 256, e, s)); }
+    NRW_TRY(mm_bwd(c, c.dNF, c.NH[8], L_NF, c.dNF, c.WT(L_NF), M, 256, 256, e, s)); }
   cur = 0;
   for (int l = 7; l >= 1; --l) {
     Planes Xin = (l == 5) ? c.IN5 : c.NH[l];
-    NRW_TRY(mm_dw(c, c.dNH[cur], Xin, M, L_N0 + l, s));
     Epi e; e.aux_relu = Xin.p; e.ld_relu = Xin.ld; e.out_pl = c.dNH[1 - cur]; e.colsum = c.db(L_N0 + l - 1);
-    NRW_TRY(mm(c, c.dNH[cur], c.WT(L_N0 + l), M, 256, 256, e, s));  // first 256 WT rows = the h part for l==5
+    // (the first 256 WT rows are the h part for l == 5)
+    NRW_TRY(mm_bwd(c, c.dNH[cur], Xin, L_N0 + l, c.dNH[cur], c.WT(L_N0 + l), M, 256, 256, e, s));
     cur = 1 - cur;
   }
   NRW_TRY(mm_dw(c, c.dNH[cur], c.IN0, M, L_N0, s));

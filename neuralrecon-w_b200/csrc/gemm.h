@@ -51,6 +51,21 @@ inline bool gemm_tc_dw_coop(const GemmDesc& g) {
          (reinterpret_cast<uintptr_t>(e.out_f32) & 7) == 0 && !e.bias && !e.rowvec && !e.out_pre && !e.colsum;
 }
 inline int gemm_tc_tile_m(const GemmDesc& g) { return gemm_tc_dw_coop(g) ? 256 : 128; }
+
+// A backward layer's data GEMM and its weight gradient, which read no output of each other: one launch runs both, so the
+// weight gradient's MMAs fill the tensor-core time the data tiles' epilogues leave idle (gemm_tc.cu, MN_PAIR).
+struct GemmPair {
+  GemmDesc data;   // K-major, one plane, 128-column tiles, non-atomic epilogue of kind GENERIC, TANGENT, REVERSE or RELU_BWD
+  GemmDesc dw;     // MN-major, one plane, N >= 128, out_f32 += scale * A^T B and nothing else; k_slices as given
+};
+// whether gemm_tc_pair runs `pr` (otherwise issue pr.dw and then pr.data as two launches)
+bool gemm_tc_pair_ok(const GemmPair& pr);
+int gemm_tc_pair(const GemmPair& pr, cudaStream_t stream);
+// K-slices of a paired weight gradient over K samples: 128 k-blocks of 64 samples per item (gemm_tc.cu header)
+inline int gemm_tc_pair_k_slices(int K) {
+  const int kb_total = cdiv(K, 64), ks = cdiv(kb_total, 128);
+  return cdiv(kb_total, cdiv(kb_total, ks));   // no empty trailing slice
+}
 // debug: when non-null, every tensor-core GEMM launch accumulates per-CTA cycle attribution into buf[SMs*16]
 void gemm_tc_set_profile_buffer(unsigned long long* buf);
 // measurement: CUDA events around every tensor-core GEMM launch (on the launching stream)

@@ -26,12 +26,26 @@
 //   barrier: each stage's empty barrier counts all 8 consumer warps.  The epilogue is one fp32 vector reduction
 //   (red.global.add.v2.f32) per accumulator pair straight from the fragment: no staging tile and no named barriers, while
 //   the producer already loads the next item's k-blocks.
+// * MN_PAIR (gemm_tc_pair): one launch runs a backward layer's data GEMM and its weight gradient together.  Work items are
+//   the 128 x 128 tiles of the one-plane K-major data GEMM (epilogue kind EK) and 128 x 128 x K-slice items of the one-plane
+//   MN-major dW.  Both fill the same 32 KB stage, so ring, stage count and barriers are those of the ping-pong schedule; the
+//   item kind (warp-uniform) selects the tensor maps, the descriptors and the epilogue: data tiles take the staged epilogue,
+//   dW items the fragment red.add of MN_COOP.  The combined list is laid out in rounds of gridDim.x items (round j = the j-th
+//   item of every CTA, so warpgroup j & 1 runs it): data and dW rounds alternate while both remain, then the rest follow.
+//   So one warpgroup runs a data tile's epilogue while the other runs a dW item's main loop on the tensor cores.  A dW
+//   round numbers its items tile-minor over consecutive K-slices: the CTAs of a round share each slice's operand slabs in L2.
+//   K-slice rule (host, gemm_tc_pair_k_slices): 128 k-blocks of 64 samples per dW item.  At the tensor-core peak a k-block
+//   is about 512 cycles, so 40 k-blocks would match a data tile's epilogue (22-25 k cycles at N = 512) minus its main loop.
+//   But both kinds stream 32 KB per k-block from L2 into shared memory, and that stream, not the tensor pipe, bounds a
+//   paired launch: longer items mean fewer items, fewer fragment reductions and fewer turn hand-overs.  Measured per C2
+//   step: 24, 40, 64 and 128 k-blocks in that order ran faster (DESIGN.md 5.1).
 #include <stdlib.h>
 
 #include <mutex>
 #include <unordered_map>
 #include <vector>
 #include <algorithm>
+#include <type_traits>
 #include <stdio.h>
 
 #include "gemm.h"
@@ -51,6 +65,7 @@ static constexpr int EPI_WG_BYTES = 64 * EPI_COLS * 4; // one warpgroup's stagin
 static constexpr int CS_BYTES = 1024;                  // column-sum accumulators: 128 columns of the current n-tile per warpgroup
 static constexpr int BAR_TURN = 4;                     // named barriers 4 + wg: warpgroup wg's turn at the tensor cores
 static constexpr int MN_COOP = 2;                      // MN_MAJOR value of the cooperative 256-row weight-gradient schedule
+static constexpr int MN_PAIR = 3;                      // MN_MAJOR value of a paired data GEMM + weight-gradient launch
 static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 32 * N_CONSUMER_WARPS <= 65536, "register file");
 static constexpr int BAR_BYTES = 256;                  // 2 x MAX_STAGES mbarriers
 static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + 2 * EPI_WG_BYTES + CS_BYTES;
@@ -70,10 +85,17 @@ struct TcParams {
   int k_slices;
   int m_tiles, n_tiles;
   Epi epi;
+  // MN_PAIR: the weight gradient, out_f32[dw_M, dw_N] += dw_scale * A2^T B2 (one plane, MN-major, split into dw_k_slices)
+  CUtensorMap tmA2, tmB2;
+  int dw_M, dw_N, dw_K, dw_k_slices, dw_m_tiles, dw_n_tiles;
+  float* dw_out;
+  int dw_ld;
+  float dw_scale;
   // optional cycle attribution (debug): per CTA 16 counters
   //  [0] producer: waiting for a free stage   [5] kernel cycles
   //  first warp of consumer warpgroup wg, o = 8 wg: [1 + o] waiting for TMA data   [3 + o] waiting for its turn at the
-  //  tensor cores   [4 + o] epilogue   [6 + o] tiles (MN_COOP: both warpgroups count every non-empty item)
+  //  tensor cores   [4 + o] epilogue   [6 + o] tiles (MN_COOP: both warpgroups count every non-empty item; MN_PAIR: data
+  //  tiles)   [7 + o] MN_PAIR: dW items
   unsigned long long* prof;
 };
 #define NRW_PROF_T0(cond) const long long _t0 = (cond) ? clock64() : 0
@@ -215,17 +237,82 @@ NRW_WGMMA_N128(0, 0)
 NRW_WGMMA_N128(1, 1)
 #undef NRW_WGMMA_N128
 
+// out[row][c] += scale * acc for the 128 rows m0 .. m0 + 127 (two m64 halves) of one warpgroup's MN-major weight-gradient
+// fragment: one red.global.add.v2.f32 per accumulator pair, masked at the M / N edges.  Fragment of warp wi in half h:
+// acc[h][4j + {0,1}] = row 64 h + 16 wi + lane / 4, columns 8 j + 2 (lane % 4) + {0,1}; acc[h][4j + {2,3}] = the same
+// columns of row + 8.
+template <int BN>
+__device__ __forceinline__ void dw_reduce(const float (&acc)[2][BN / 2], float* out, int ld, float scale, int m0, int n0,
+                                          int M, int n_lim, int wi, int lane) {
+  const int c0 = n0 + 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int r8 = 0; r8 < 2; ++r8) {
+      const int row = m0 + 64 * h + 16 * wi + (lane >> 2) + 8 * r8;
+      if (row >= M) continue;
+      float* dst = out + (long long)row * ld;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = c0 + 8 * j;
+        const float x0 = acc[h][4 * j + 2 * r8] * scale, x1 = acc[h][4 * j + 2 * r8 + 1] * scale;
+        if (c + 1 < n_lim) red_add_v2(dst + c, x0, x1);
+        else if (c < n_lim) atomicAdd(dst + c, x0);
+      }
+    }
+}
+
+// One work item of a CTA: output tile origin, k-block range [kb0, kb1) (empty: kb1 <= kb0), and for MN_PAIR its kind.
+struct TcItem { int m0, n0, kb0, kb1; bool dw; };
+
+// item j of this CTA.  Plain launches: item blockIdx.x + j gridDim.x of the slice-minor list.  MN_PAIR: round j (see the
+// header comment); positions past the end of a kind's last round are empty items.
+template <int BN, int TM, bool PAIR>
+__device__ __forceinline__ TcItem tc_item(const TcParams& p, int j, int kb_total, int kb_per) {
+  TcItem it;
+  it.dw = false;
+  if constexpr (PAIR) {
+    const int G = gridDim.x;
+    const int n_data = p.m_tiles * p.n_tiles, dw_tiles = p.dw_m_tiles * p.dw_n_tiles, n_dw = dw_tiles * p.dw_k_slices;
+    const int rd = (n_data + G - 1) / G, rw = (n_dw + G - 1) / G, ri = min(rd, rw);
+    int r;
+    if (j < 2 * ri) { it.dw = (j & 1) != 0; r = j >> 1; }
+    else { it.dw = rd <= ri; r = j - ri; }
+    const int i = r * G + blockIdx.x;
+    if (!it.dw) {
+      it.n0 = (i % p.n_tiles) * BN; it.m0 = (i / p.n_tiles) * BM;
+      it.kb0 = 0; it.kb1 = i < n_data ? kb_total : 0;
+    } else {
+      const int t = i % dw_tiles, ks = i / dw_tiles;
+      const int dw_kb_total = (p.dw_K + BK - 1) / BK, dw_kb_per = (dw_kb_total + p.dw_k_slices - 1) / p.dw_k_slices;
+      it.n0 = (t % p.dw_n_tiles) * BN; it.m0 = (t / p.dw_n_tiles) * BM;
+      it.kb0 = ks * dw_kb_per; it.kb1 = i < n_dw ? min(dw_kb_total, it.kb0 + dw_kb_per) : 0;
+    }
+    return it;
+  }
+  const int item = blockIdx.x + j * gridDim.x;
+  const int ks = item % p.k_slices;
+  const int t = item / p.k_slices;
+  it.n0 = (t % p.n_tiles) * BN; it.m0 = (t / p.n_tiles) * TM;
+  it.kb0 = ks * kb_per; it.kb1 = min(kb_total, it.kb0 + kb_per);
+  return it;
+}
+
 // product p of the plane expansion -> (a_plane, b_plane); ordered small-to-large magnitude last
 //   n_planes==1: (0,0); ==2: (0,1),(1,0),(0,0); ==3: (0,2),(2,0),(1,1),(0,1),(1,0),(0,0)
 // With q = n_products-1-p (q=0 is (hi,hi)): a_plane = nibble q of 0x021010, b_plane = nibble q of 0x201100.
 
 // EK: compile-time epilogue kind (epilogue_fast.cuh); MN-major launches use EK_GENERIC.  MN_MAJOR: 0 K-major, 1 MN-major
-// ping-pong, MN_COOP MN-major with 256-row items shared by both warpgroups.
+// ping-pong, MN_COOP MN-major with 256-row items shared by both warpgroups, MN_PAIR K-major data tiles (kind EK) and
+// MN-major weight-gradient items in one ping-pong launch.
 template <int BN, int MN_MAJOR, int EK>
 __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
   static_assert(BN == 64 || BN == 128, "wgmma tile width");
   constexpr bool COOP = MN_MAJOR == MN_COOP;
+  constexpr bool PAIR = MN_MAJOR == MN_PAIR;
+  constexpr int TR = MN_MAJOR == 1 ? 1 : 0;     // transpose flag of the (data) wgmma operands
   static_assert(!COOP || (BN == 128 && EK == EK_GENERIC), "the cooperative schedule is the 256 x 128 weight-gradient tile");
+  static_assert(!PAIR || BN == 128, "paired launches run 128 x 128 items of both kinds");
   constexpr int TM = COOP ? 2 * BM : BM;        // rows of a work item
   constexpr int A_TILE = TM * BK * 2;
   constexpr int B_TILE = BN * BK * 2;
@@ -250,6 +337,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       tma_prefetch_desc(&p.tmA[i]);
       tma_prefetch_desc(&p.tmB[i]);
     }
+    if (PAIR) {
+      tma_prefetch_desc(&p.tmA2);
+      tma_prefetch_desc(&p.tmB2);
+    }
     for (int i = 0; i < MAX_STAGES; ++i) {
       mbar_init(bar_full + 8 * i, 1);
       mbar_init(bar_empty + 8 * i, COOP ? 8 : 4);   // the four warps of the stage's consuming warpgroup (COOP: both)
@@ -265,6 +356,13 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
   const int kb_per = (kb_total + p.k_slices - 1) / p.k_slices;
   const int n_items = p.m_tiles * p.n_tiles * p.k_slices;
   const int n_prod = (P == 1) ? 1 : (P == 2 ? 3 : 6);
+  int n_j;   // items of this CTA (MN_PAIR: rounds, empty items included)
+  if constexpr (PAIR) {
+    const int G = gridDim.x, n_dw = p.dw_m_tiles * p.dw_n_tiles * p.dw_k_slices;
+    n_j = (n_items + G - 1) / G + (n_dw + G - 1) / G;
+  } else {
+    n_j = (n_items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  }
 
   if (warp >= N_CONSUMER_WARPS) {
     // ===================== TMA producer: every item's k-blocks in item order =====================
@@ -272,12 +370,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     if (warp == N_CONSUMER_WARPS && lane == 0) {
       int s = 0;
       uint32_t ph = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int ks = item % p.k_slices;
-        const int t = item / p.k_slices;
-        const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * TM;
-        const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
-        for (int kb = kb0; kb < kb1; ++kb) {
+      for (int j = 0; j < n_j; ++j) {
+        const TcItem it = tc_item<BN, TM, PAIR>(p, j, kb_total, kb_per);
+        const int n0 = it.n0, m0 = it.m0;
+        for (int kb = it.kb0; kb < it.kb1; ++kb) {
           {
             NRW_PROF_T0(p.prof != nullptr);
             mbar_wait(bar_empty + 8 * s, ph ^ 1);
@@ -286,8 +382,14 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
           mbar_arrive_expect_tx(bar_full + 8 * s, stage_bytes);
           const uint32_t sa = smem_u32(smem + s * stage_bytes);
           const uint32_t sb = sa + P * A_TILE;
-          for (int pl = 0; pl < P; ++pl) {
-            if (MN_MAJOR == 0) {
+          if (PAIR && it.dw) {                         // MN-major weight-gradient k-block: two 64-wide slabs of each operand
+#pragma unroll
+            for (int sl = 0; sl < 2; ++sl) {
+              tma_load_2d(sa + sl * (64 * BK * 2), &p.tmA2, bar_full + 8 * s, m0 + 64 * sl, kb * BK);
+              tma_load_2d(sb + sl * (64 * BK * 2), &p.tmB2, bar_full + 8 * s, n0 + 64 * sl, kb * BK);
+            }
+          } else for (int pl = 0; pl < P; ++pl) {
+            if (MN_MAJOR == 0 || PAIR) {
               tma_load_2d(sa + pl * A_TILE, &p.tmA[pl], bar_full + 8 * s, kb * BK, m0);
               tma_load_2d(sb + pl * B_TILE, &p.tmB[pl], bar_full + 8 * s, kb * BK, n0);
             } else {
@@ -367,24 +469,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       if (kb1 <= kb0) continue;                           // an empty K-slice stores nothing
       NRW_PROF_T0(prof);
       if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6 + po], 1ull);
-      // fragment of warp wi in half h: acc[h][4j + {0,1}] = row 128 wg + 64 h + 16 wi + lane / 4, columns 8 j + 2 (lane % 4)
-      // + {0,1}; acc[h][4j + {2,3}] = the same columns of row + 8
-      const int c0 = n0 + 2 * (lane & 3);
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int r8 = 0; r8 < 2; ++r8) {
-          const int row = m0 + 128 * wg + 64 * h + 16 * wi + (lane >> 2) + 8 * r8;
-          if (row >= p.M) continue;
-          float* dst = p.epi.out_f32 + (long long)row * p.epi.ld_f32;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const int c = c0 + 8 * j;
-            const float x0 = acc[h][4 * j + 2 * r8] * p.epi.scale, x1 = acc[h][4 * j + 2 * r8 + 1] * p.epi.scale;
-            if (c + 1 < n_lim) red_add_v2(dst + c, x0, x1);
-            else if (c < n_lim) atomicAdd(dst + c, x0);
-          }
-        }
+      dw_reduce<BN>(acc, p.epi.out_f32, p.epi.ld_f32, p.epi.scale, m0 + 128 * wg, n0, p.M, n_lim, wi, lane);
       NRW_PROF_ADD(prof, 4 + po);
     }
   } else {
@@ -393,9 +478,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     const int wg = warp >> 2, wi = warp & 3;
     const uint32_t smem0 = smem_u32(smem);
     // K-major: SBO = 8 rows * 128 B; MN-major: LBO = stride between 64-wide MN slabs, SBO = 8 k-rows
-    constexpr uint32_t LBO = MN_MAJOR ? (64 * BK * 2) : 16;
+    constexpr uint32_t LBO = TR ? (64 * BK * 2) : 16;
     constexpr uint32_t SBO = 1024;
-    constexpr uint32_t KSTEP = MN_MAJOR ? (16 * 128) : 32;  // bytes per wgmma K=16
+    constexpr uint32_t KSTEP = TR ? (16 * 128) : 32;         // bytes per wgmma K=16
+    constexpr uint32_t KSTEP_DW = 16 * 128;                  // MN_PAIR weight-gradient items (MN-major)
     const uint64_t desc_hi = make_gdesc(0, LBO, SBO);         // everything but the start address
     float* stage_tile = epi_buf + wg * (EPI_WG_BYTES / 4);
     const bool use_cs = p.epi.colsum != nullptr && !p.epi.atomic;
@@ -407,18 +493,16 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     int s = 0;        // ring position (stage, phase) of the next k-block, over every item of the CTA
     uint32_t ph = 0;
     // item j of the CTA: items of both warpgroups are walked so that the ring position stays in step with the producer
-    for (int j = 0; blockIdx.x + j * gridDim.x < n_items; ++j) {
-      const int item = blockIdx.x + j * gridDim.x;
-      const int ks = item % p.k_slices;
-      const int t = item / p.k_slices;
-      const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * BM;
-      const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
+    for (int j = 0; j < n_j; ++j) {
+      const TcItem it = tc_item<BN, BM, PAIR>(p, j, kb_total, kb_per);
+      const int n0 = it.n0, m0 = it.m0, kb0 = it.kb0, kb1 = it.kb1;
+      const bool dw = PAIR && it.dw;                         // warp-uniform: a weight-gradient item of a paired launch
       if ((j & 1) != wg) {                                   // the other warpgroup's item: skip its stages
         for (int kb = kb0; kb < kb1; ++kb)
           if (++s == stages) { s = 0; ph ^= 1; }
         continue;
       }
-      if (use_cs && n0 != cs_n0) {
+      if (use_cs && !dw && n0 != cs_n0) {
         if (cs_n0 >= 0) colsum_flush(cs_wg, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 128, 2 + wg);
         cs_n0 = n0;
       }
@@ -435,49 +519,73 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
         named_bar_sync(BAR_TURN + wg, 256);
         NRW_PROF_ADD(prof, 3 + po);
       }
-      int prev_s = -1;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        {
-          NRW_PROF_T0(prof);
-          mbar_wait(bar_full + 8 * s, ph);
-          NRW_PROF_ADD(prof, 1 + po);
-        }
-        const uint32_t sa = smem0 + s * stage_bytes;
-        const uint32_t sb = smem0 + s * stage_bytes + P * A_TILE;
-        wgmma_fence();
-        for (int pr = 0; pr < n_prod; ++pr) {
-          const int q = 4 * (n_prod - 1 - pr);           // product order of product_planes(), packed lookup
-          const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
-          const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE) & 0x3FFFFu) >> 4);
-          const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
+      // The main loop, instantiated once per item kind (DW: a weight-gradient item of a paired launch, MN-major operands).
+      // Each kind's wgmma sequence, from the first fence to the final wait, lies on one path: wgmma variants that share
+      // accumulators under a per-k-block branch would make ptxas serialise every wgmma of the kernel.
+      auto main_loop = [&](auto kind) {
+        constexpr bool DW = decltype(kind)::value;
+        int prev_s = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          {
+            NRW_PROF_T0(prof);
+            mbar_wait(bar_full + 8 * s, ph);
+            NRW_PROF_ADD(prof, 1 + po);
+          }
+          const uint32_t sa = smem0 + s * stage_bytes;
+          const uint32_t sb = smem0 + s * stage_bytes + P * A_TILE;
+          wgmma_fence();
+          if constexpr (DW) {                            // one plane, both operands MN-major
+            const uint64_t desc_dw = make_gdesc(0, 64 * BK * 2, SBO);
+            const uint64_t da = desc_dw | (uint64_t)((sa & 0x3FFFFu) >> 4);
+            const uint64_t db = desc_dw | (uint64_t)((sb & 0x3FFFFu) >> 4);
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
+            for (int k = 0; k < BK / 16; ++k)
 #pragma unroll
-            for (int h = 0; h < 2; ++h)                  // 64-row half h: K-major rows at +8 KB, or the second MN-major slab
-              wgmma_bf16<BN, MN_MAJOR, MN_MAJOR>(acc[h], da + ((h * WG_A + k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
-        }
-        wgmma_commit();
-        acc_fence(acc[0]);
-        acc_fence(acc[1]);
-        if (prev_s >= 0) {                                // the previous stage's MMAs have completed: hand it back
-          wgmma_wait<1>();
+              for (int h = 0; h < 2; ++h)
+                wgmma_bf16<BN, 1, 1>(acc[h], da + ((h * WG_A + k * KSTEP_DW) >> 4), db + ((k * KSTEP_DW) >> 4), 1u);
+          } else {
+            for (int pr = 0; pr < n_prod; ++pr) {
+              const int q = 4 * (n_prod - 1 - pr);         // product order of product_planes(), packed lookup
+              const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
+              const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE) & 0x3FFFFu) >> 4);
+              const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
+#pragma unroll
+              for (int k = 0; k < BK / 16; ++k)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)                // 64-row half h: K-major rows at +8 KB, or the second MN-major slab
+                  wgmma_bf16<BN, TR, TR>(acc[h], da + ((h * WG_A + k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
+            }
+          }
+          wgmma_commit();
           acc_fence(acc[0]);
           acc_fence(acc[1]);
-          if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+          if (prev_s >= 0) {                              // the previous stage's MMAs have completed: hand it back
+            wgmma_wait<1>();
+            acc_fence(acc[0]);
+            acc_fence(acc[1]);
+            if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+          }
+          prev_s = s;
+          if (++s == stages) { s = 0; ph ^= 1; }
         }
-        prev_s = s;
-        if (++s == stages) { s = 0; ph ^= 1; }
-      }
-      // every MMA of this item is issued: the other warpgroup's main loop may start (if the CTA has an item j+1)
-      if (item + gridDim.x < n_items) named_bar_arrive(BAR_TURN + (wg ^ 1), 256);
-      wgmma_wait<0>();
-      acc_fence(acc[0]);
-      acc_fence(acc[1]);
-      if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+        // every MMA of this item is issued: the other warpgroup's main loop may start (if the CTA has an item j+1)
+        if (j + 1 < n_j) named_bar_arrive(BAR_TURN + (wg ^ 1), 256);
+        wgmma_wait<0>();
+        acc_fence(acc[0]);
+        acc_fence(acc[1]);
+        if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
+      };
+      if (dw) main_loop(std::true_type{});
+      else main_loop(std::false_type{});
       // (an empty k-slice accumulates nothing and stores nothing)
       if (kb1 <= kb0) continue;
       NRW_PROF_T0(prof);
-      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6 + po], 1ull);
+      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + (dw ? 7 : 6) + po], 1ull);
+      if (dw) {
+        dw_reduce<BN>(acc, p.dw_out, p.dw_ld, p.dw_scale, m0, n0, p.dw_M, p.dw_N, wi, lane);
+        NRW_PROF_ADD(prof, 4 + po);
+        continue;
+      }
       // ---- epilogue, per 64-row half h: 64 columns per round through the warpgroup's staging tile.  Fragment of warp wi:
       // acc[h][4j + {0,1}] = row 64 h + 16 wi + lane / 4, columns 8 j + 2 (lane % 4) + {0,1}; acc[h][4j + {2,3}] = the same columns
       // of row + 8.  After the barrier warp wi reads rows 64 h + 32 (wi & 1) .. +31 and columns 16 (wi >> 1) .. +15 (chunk 0) and
@@ -650,7 +758,7 @@ static int launch(const TcParams& p, int n_sm, int dev, cudaStream_t stream) {
     NRW_CUDA_OK((cudaFuncSetAttribute(gemm_tc_kernel<BN, MN, EK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)));
     attr_set[dev] = true;
   }
-  const int items = p.m_tiles * p.n_tiles * p.k_slices;
+  const int items = p.m_tiles * p.n_tiles * p.k_slices + (MN == MN_PAIR ? p.dw_m_tiles * p.dw_n_tiles * p.dw_k_slices : 0);
   const int grid = items < n_sm ? items : n_sm;
   NRW_CUDA_OK((launch_gemm(gemm_tc_kernel<BN, MN, EK>, grid, N_THREADS, stream, p)));
   NRW_LAUNCH_OK();
@@ -661,7 +769,12 @@ static int launch(const TcParams& p, int n_sm, int dev, cudaStream_t stream) {
 static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream);
 
 // ---- live kernel timing (bench.py roofline): CUDA events around every launch on the launching stream ----
-struct TimedLaunch { cudaEvent_t e0, e1; double flops; double mma_flops; int M, N, K, P, mn, ks; unsigned epi; double bytes; };
+// (a paired launch records its data GEMM's shape and epilogue in M .. epi and its weight gradient's in M2, N2, K2, ks2; flops,
+// mma_flops and bytes are the sums of both)
+struct TimedLaunch {
+  cudaEvent_t e0, e1; double flops; double mma_flops; int M, N, K, P, mn, ks; unsigned epi; double bytes;
+  int M2 = 0, N2 = 0, K2 = 0, ks2 = 0;
+};
 static std::vector<TimedLaunch> g_timed;
 static std::vector<cudaEvent_t> g_event_pool;
 static bool g_timing_on = false;
@@ -677,6 +790,7 @@ int gemm_tc_timing_read(double* ms, double* flops, double* mma_flops, long long*
   double t = 0, f = 0, mf = 0, by = 0;
   // tuning: NRW_GEMM_TIMING_DUMP=<path> appends one CSV row per launch: M,N,K,planes,mn_major,k_slices,epilogue bits,
   // algorithmic bytes,ms   (bits: 1 out_pre 2 out_f32 4 out2 8 planes 16 gate (aux_u) 32 aux_q 64 aux_add 128 aux_relu 256 atomic 512 colsum)
+  // A paired launch (mn_major 3) appends its weight gradient's M,N,K,k_slices; bytes and ms cover both GEMMs.
   FILE* dump = getenv("NRW_GEMM_TIMING_DUMP") ? fopen(getenv("NRW_GEMM_TIMING_DUMP"), "a") : nullptr;
   for (auto& L : g_timed) {
     NRW_CUDA_OK(cudaEventSynchronize(L.e1));
@@ -684,7 +798,10 @@ int gemm_tc_timing_read(double* ms, double* flops, double* mma_flops, long long*
     NRW_CUDA_OK(cudaEventElapsedTime(&dt, L.e0, L.e1));
     t += dt; f += L.flops; mf += L.mma_flops; by += L.bytes;
     g_event_pool.push_back(L.e0); g_event_pool.push_back(L.e1);
-    if (dump) fprintf(dump, "%d,%d,%d,%d,%d,%d,%u,%.0f,%.4f\n", L.M, L.N, L.K, L.P, L.mn, L.ks, L.epi, L.bytes, dt);
+    if (dump && L.mn == MN_PAIR)
+      fprintf(dump, "%d,%d,%d,%d,%d,%d,%u,%.0f,%.4f,%d,%d,%d,%d\n", L.M, L.N, L.K, L.P, L.mn, L.ks, L.epi, L.bytes, dt, L.M2, L.N2,
+              L.K2, L.ks2);
+    else if (dump) fprintf(dump, "%d,%d,%d,%d,%d,%d,%u,%.0f,%.4f\n", L.M, L.N, L.K, L.P, L.mn, L.ks, L.epi, L.bytes, dt);
   }
   if (dump) fclose(dump);
   *ms = t; *flops = f; *mma_flops = mf; *launches = (long long)g_timed.size();
@@ -693,35 +810,112 @@ int gemm_tc_timing_read(double* ms, double* flops, double* mma_flops, long long*
   return NRW_OK;
 }
 
-int gemm_tc(const GemmDesc& g, cudaStream_t stream) {
-  if (!g_timing_on) return gemm_tc_impl(g, stream);
-  TimedLaunch L;
-  L.e0 = get_event(); L.e1 = get_event();
-  L.flops = 2.0 * g.M * g.N * g.K;
-  L.mma_flops = L.flops * n_products(g.n_planes);
-  L.M = g.M; L.N = g.N; L.K = g.K; L.P = g.n_planes; L.mn = g.mn_major; L.ks = g.k_slices;
+// adds g's algorithmic FLOP, MMA FLOP and bytes to L
+static void account(const GemmDesc& g, TimedLaunch& L) {
+  L.flops += 2.0 * g.M * g.N * g.K;
+  L.mma_flops += 2.0 * g.M * g.N * g.K * n_products(g.n_planes);
   const Epi& e = g.epi;
   const int q_bytes = e.aux_q_bcast ? 0 : e.aux_q.elem_bytes();   // a broadcast row vector is no stream
+  const double mn = (double)g.M * (double)std::min(g.N, e.n_store);
+  L.bytes += 2.0 * g.n_planes * ((double)g.M * g.K + (double)g.N * g.K) + (double)e.out_pre.elem_bytes() * g.M * g.N +
+             mn * (4.0 * (e.out_f32 ? 1 : 0) + e.out2.elem_bytes() + q_bytes + e.aux_add.elem_bytes() + 2.0 * e.n_planes +
+                   (e.aux_relu ? 2.0 : 0.0) + (e.aux_u.p ? 2.0 * e.aux_u_planes : 0.0));
+}
+static TimedLaunch timed_launch(const GemmDesc& g) {
+  TimedLaunch L;
+  L.e0 = get_event(); L.e1 = get_event();
+  L.flops = L.mma_flops = L.bytes = 0.0;
+  account(g, L);
+  L.M = g.M; L.N = g.N; L.K = g.K; L.P = g.n_planes; L.mn = g.mn_major; L.ks = g.k_slices;
+  const Epi& e = g.epi;
+  const int q_bytes = e.aux_q_bcast ? 0 : e.aux_q.elem_bytes();
   L.epi = (e.out_pre ? 1u : 0u) | (e.out_f32 ? 2u : 0u) | (e.out2 ? 4u : 0u) | (e.n_planes ? 8u : 0u) | (e.aux_u.p ? 16u : 0u) |
           (q_bytes ? 32u : 0u) | (e.aux_add ? 64u : 0u) | (e.aux_relu ? 128u : 0u) | (e.atomic ? 256u : 0u) | (e.colsum ? 512u : 0u);
-  const double mn = (double)g.M * (double)std::min(g.N, e.n_store);
-  L.bytes = 2.0 * g.n_planes * ((double)g.M * g.K + (double)g.N * g.K) + (double)e.out_pre.elem_bytes() * g.M * g.N +
-            mn * (4.0 * (e.out_f32 ? 1 : 0) + e.out2.elem_bytes() + q_bytes + e.aux_add.elem_bytes() + 2.0 * e.n_planes +
-                  (e.aux_relu ? 2.0 : 0.0) + (e.aux_u.p ? 2.0 * e.aux_u_planes : 0.0));
+  return L;
+}
+
+int gemm_tc(const GemmDesc& g, cudaStream_t stream) {
+  if (!g_timing_on) return gemm_tc_impl(g, stream);
+  TimedLaunch L = timed_launch(g);
   NRW_CUDA_OK(cudaEventRecord(L.e0, stream));
   const int rc = gemm_tc_impl(g, stream);
   NRW_CUDA_OK(cudaEventRecord(L.e1, stream));
   g_timed.push_back(L);
   return rc;
 }
+
+static int sm_count(int dev, int& n_sm) {
+  static int n_sm_dev[MAX_DEV] = {0};
+  if (!n_sm_dev[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm_dev[dev], cudaDevAttrMultiProcessorCount, dev));
+  n_sm = n_sm_dev[dev];
+  return NRW_OK;
+}
+
+// weight gradients that run as the fragment red.add epilogue: out_f32 += scale * A^T B and nothing else, 8-byte aligned rows
+static bool dw_only(const GemmDesc& g) {
+  const Epi& e = g.epi;
+  return g.mn_major && e.atomic && e.out_f32 && e.ld_f32 % 2 == 0 && (reinterpret_cast<uintptr_t>(e.out_f32) & 7) == 0 &&
+         e.act == ACT_NONE && !e.bias && !e.rowvec && !e.colvec && !e.aux_u.p && !e.aux_q && !e.aux_add && !e.aux_relu && !e.out_pre && !e.out2 &&
+         !e.out_pl.p && !e.n_planes && !e.colsum && !e.head_w && !e.head_partial;
+}
+
+bool gemm_tc_pair_ok(const GemmPair& pr) {
+  const GemmDesc &d = pr.data, &w = pr.dw;
+  const int ek = d.mn_major ? -1 : pick_epi_kind(d.epi);
+  return d.n_planes == 1 && w.n_planes == 1 && d.k_slices == 1 && !d.epi.atomic && gemm_tc_tile_n(d.N) == 128 &&
+         (ek == EK_GENERIC || ek == EK_TANGENT || ek == EK_REVERSE || ek == EK_RELU_BWD) && w.N >= 128 && dw_only(w);
+}
+
+static int gemm_tc_pair_impl(const GemmPair& pr, cudaStream_t stream) {
+  const GemmDesc &d = pr.data, &w = pr.dw;
+  NRW_CHECK(d.M > 0 && d.N > 0 && d.K > 0 && w.M > 0 && w.N > 0 && w.K > 0 && w.k_slices >= 1, NRW_ERR_ARG,
+            "gemm_tc_pair: empty problem %d %d %d / %d %d %d", d.M, d.N, d.K, w.M, w.N, w.K);
+  NRW_CHECK(gemm_tc_pair_ok(pr), NRW_ERR_ARG, "gemm_tc_pair: the two GEMMs cannot share a launch");
+  NRW_CHECK(d.K % BK == 0, NRW_ERR_ARG, "gemm_tc_pair: K=%d must be a multiple of %d (pad the operand)", d.K, BK);
+  const int dev = current_device();
+  int n_sm = 0;
+  NRW_TRY(sm_count(dev, n_sm));
+  TcParams p;
+  memset(&p, 0, sizeof(p));
+  p.M = d.M; p.N = d.N; p.K = d.K; p.n_planes = 1; p.k_slices = 1;
+  p.m_tiles = cdiv(d.M, BM); p.n_tiles = cdiv(d.N, 128);
+  p.epi = d.epi;
+  p.prof = g_prof_ptr;
+  NRW_TRY(make_map(&p.tmA[0], d.A.plane(0), d.K, d.M, d.A.ld, BK, BM));
+  NRW_TRY(make_map(&p.tmB[0], d.B.plane(0), d.K, d.N, d.B.ld, BK, 128));
+  NRW_TRY(make_map(&p.tmA2, w.A.plane(0), w.M, w.K, w.A.ld, 64, BK));
+  NRW_TRY(make_map(&p.tmB2, w.B.plane(0), w.N, w.K, w.B.ld, 64, BK));
+  p.dw_M = w.M; p.dw_N = std::min(w.N, w.epi.n_store); p.dw_K = w.K; p.dw_k_slices = w.k_slices;
+  p.dw_m_tiles = cdiv(w.M, BM); p.dw_n_tiles = cdiv(w.N, 128);
+  p.dw_out = w.epi.out_f32; p.dw_ld = w.epi.ld_f32; p.dw_scale = w.epi.scale;
+  switch (pick_epi_kind(d.epi)) {
+    case EK_TANGENT: return launch<128, MN_PAIR, EK_TANGENT>(p, n_sm, dev, stream);
+    case EK_REVERSE: return launch<128, MN_PAIR, EK_REVERSE>(p, n_sm, dev, stream);
+    case EK_RELU_BWD: return launch<128, MN_PAIR, EK_RELU_BWD>(p, n_sm, dev, stream);
+    default: return launch<128, MN_PAIR, EK_GENERIC>(p, n_sm, dev, stream);
+  }
+}
+
+int gemm_tc_pair(const GemmPair& pr, cudaStream_t stream) {
+  if (!g_timing_on) return gemm_tc_pair_impl(pr, stream);
+  TimedLaunch L = timed_launch(pr.data);
+  account(pr.dw, L);
+  L.mn = MN_PAIR;
+  L.M2 = pr.dw.M; L.N2 = pr.dw.N; L.K2 = pr.dw.K; L.ks2 = pr.dw.k_slices;
+  NRW_CUDA_OK(cudaEventRecord(L.e0, stream));
+  const int rc = gemm_tc_pair_impl(pr, stream);
+  NRW_CUDA_OK(cudaEventRecord(L.e1, stream));
+  g_timed.push_back(L);
+  return rc;
+}
+
 static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
   NRW_CHECK(g.M > 0 && g.N > 0 && g.K > 0, NRW_ERR_ARG, "gemm_tc: empty problem %d %d %d", g.M, g.N, g.K);
   NRW_CHECK(g.n_planes >= 1 && g.n_planes <= 3, NRW_ERR_ARG, "gemm_tc: n_planes=%d", g.n_planes);
   NRW_CHECK(g.k_slices == 1 || g.epi.atomic, NRW_ERR_ARG, "gemm_tc: split-K needs an atomic epilogue");
-  static int n_sm_dev[MAX_DEV] = {0};
   const int dev = current_device();
-  if (!n_sm_dev[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm_dev[dev], cudaDevAttrMultiProcessorCount, dev));
-  const int n_sm = n_sm_dev[dev];
+  int n_sm = 0;
+  NRW_TRY(sm_count(dev, n_sm));
   // 128 x 128 tiles (one warpgroup, two m64n128 halves): with two operand planes that is 64 KB per k-block and 3 TMA stages
   const int BN = gemm_tc_tile_n(g.N);
   const bool coop = gemm_tc_dw_coop(g);

@@ -149,6 +149,7 @@ def lib():
     L.nrw_gemm_test_scratch_bytes.restype = ll
     L.nrw_gemm_test_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_gemm_test.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp]
+    L.nrw_gemm_pair_test.argtypes = [i32] * 9 + [vp] * 8 + [f32, i32] + [vp] * 6
     L.nrw_launch_count.restype = ll
     L.nrw_debug_gemm_profile.argtypes = [vp]
     L.nrw_gemm_timing.argtypes = [i32, C.POINTER(C.c_double)]
@@ -161,7 +162,7 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_pack_weights", "nrw_sdf_query", "nrw_neuconw_forward", "nrw_nerf_forward", "nrw_sample",
            "nrw_samples_per_ray", "nrw_upsample_round", "nrw_render_forward", "nrw_render_backward",
            "nrw_composite_forward", "nrw_composite_backward", "nrw_octree_near_far", "nrw_octree_hits",
-           "nrw_gemm_test_scratch_bytes", "nrw_gemm_test", "nrw_launch_count", "nrw_debug_gemm_profile",
+           "nrw_gemm_test_scratch_bytes", "nrw_gemm_test", "nrw_gemm_pair_test", "nrw_launch_count", "nrw_debug_gemm_profile",
            "nrw_gemm_timing", "nrw_ctx_set_backward_planes", "nrw_octree_build_scratch_bytes", "nrw_octree_build",
            "nrw_grad_sumsq", "nrw_adam_clip_step", "nrw_boundary_samples", "nrw_compact_scratch_bytes", "nrw_raycache_gather",
            "nrw_grid_points_dense", "nrw_grid_points_sparse", "nrw_threshold_compact", "nrw_ctx_set_backward_gate_planes",

@@ -31,7 +31,9 @@ kern = s[5]
 print(f"{precision}: kernel cycles summed over CTAs {kern:.4g}; producer waiting for a free stage {100 * s[0] / kern:.1f} %")
 for wg in range(2):
     o = 8 * wg
-    if s[6 + o] == 0:
+    n = s[6 + o] + s[7 + o]
+    if n == 0:
         continue
-    print(f"  warpgroup {wg}: tiles {s[6 + o]:.0f}  TMA wait {100 * s[1 + o] / kern:5.1f} %  tensor-core turn wait {100 * s[3 + o] / kern:5.1f} %"
-          f"  epilogue {100 * s[4 + o] / kern:5.1f} %  epilogue per tile {s[4 + o] / s[6 + o]:.0f} cycles")
+    print(f"  warpgroup {wg}: tiles {s[6 + o]:.0f}  paired dW items {s[7 + o]:.0f}  TMA wait {100 * s[1 + o] / kern:5.1f} %"
+          f"  tensor-core turn wait {100 * s[3 + o] / kern:5.1f} %  epilogue {100 * s[4 + o] / kern:5.1f} %"
+          f"  epilogue per item {s[4 + o] / n:.0f} cycles")
