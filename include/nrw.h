@@ -401,6 +401,25 @@ NRW_API int nrw_view_roi_count(const float* views, const int32_t* hw, int n_view
 NRW_API int nrw_label_static_count(const float* labels, long long n, const int32_t* ids_host, int n_ids, int64_t* count,
                                    void* stream);
 
+/* ---- ground-truth alignment check (tools/reproj_error.py; rules in csrc/gtproj.cu) -------------------------------
+ * nrw_first_hit writes hit (device int64 [n_queries]): for each query (q_view int32, q_xy f32 [n_queries, 2], both on
+ * the device) the index of the point (f32 [n_points, 3], n_points < 2^32) with the smallest fp32 camera depth > 0 whose
+ * fp64 projection rounds to the query's pixel (rint of its xy), the smaller index on equal depths, or -1.  views (HOST
+ * f64 [n_views, 16]) = world->camera [3, 4] row-major, fx, fy, cx, cy; boxes (HOST int32 [n_views, 4]) = x0, y0, width,
+ * height of the bounding box of each view's query pixels (width or height 0 for a view without queries).  A query whose
+ * view is out of range or whose pixel lies outside its box gets -1 and sets bit 0 of status (device int32, cleared).
+ * scratch (256-byte aligned) of scratch_bytes >= nrw_first_hit_scratch_bytes(n_queries, largest box area); a larger
+ * scratch fits more views into one pass over the points.  The result does not depend on the pass layout.
+ * nrw_obs_reproj_error writes err (device f64 [n]): the distance of the projection of X (f64 [n, 3]) by the P = K [R|t]
+ * (device f64 [n_views, 12]) of view[i] (int32 [n]) to xy (f64 [n, 2]); uv (f64 [n, 2], nullable) receives the
+ * projection.  An out-of-range view gives NaN.  Every argument is checked before any launch; nothing is read back. */
+NRW_API long long nrw_first_hit_scratch_bytes(long long n_queries, long long map_pixels);
+NRW_API int nrw_first_hit(const float* points, long long n_points, const double* views_host, const int32_t* boxes_host,
+                          int n_views, const int32_t* q_view, const float* q_xy, long long n_queries, int64_t* hit,
+                          int32_t* status, void* scratch, long long scratch_bytes, void* stream);
+NRW_API int nrw_obs_reproj_error(const double* X, const int32_t* view, const double* xy, long long n, const double* P,
+                                 int n_views, double* err, double* uv, void* stream);
+
 /* ---- unit-test hooks ---------------------------------------------------------------------- */
 /* D[M,N] = (sum planes of A)[M,K] * (sum planes of B)[N,K]^T from fp32 inputs: splits into planes in
  * scratch (caller-provided, nrw_gemm_test_scratch_bytes) and runs the selected backend. */

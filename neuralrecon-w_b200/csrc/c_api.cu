@@ -437,6 +437,23 @@ long long nrw_gemm_test_scratch_bytes(int M, int N, int K) {
   const long long a = round_up((long long)M * K, 512), b = round_up((long long)N * K, 512);
   return (a + b) * 3 * 2 + 4096;
 }
+long long nrw_first_hit_scratch_bytes(long long n_queries, long long map_pixels) {
+  return first_hit_scratch_bytes(n_queries, map_pixels);
+}
+int nrw_first_hit(const float* points, long long n_points, const double* views_host, const int32_t* boxes_host, int n_views,
+                  const int32_t* q_view, const float* q_xy, long long n_queries, int64_t* hit, int32_t* status,
+                  void* scratch, long long scratch_bytes, void* stream) {
+  NRW_GUARD_BEGIN
+  return first_hit(points, n_points, views_host, boxes_host, n_views, q_view, q_xy, n_queries, hit, status, scratch,
+                   scratch_bytes, S(stream));
+  NRW_GUARD_END
+}
+int nrw_obs_reproj_error(const double* X, const int32_t* view, const double* xy, long long n, const double* P, int n_views,
+                         double* err, double* uv, void* stream) {
+  NRW_GUARD_BEGIN
+  return obs_reproj_error(X, view, xy, n, P, n_views, err, uv, S(stream));
+  NRW_GUARD_END
+}
 int nrw_gemm_test(int backend, int n_planes, int mn_major, int k_slices, int M, int N, int K, const float* A,
                   const float* B, const float* bias, int act, float* D, void* scratch, void* stream) {
   NRW_GUARD_BEGIN

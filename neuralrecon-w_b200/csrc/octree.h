@@ -109,3 +109,13 @@ int view_roi_count(const float* views, const int32_t* hw, int n_views, long long
                    int64_t* counts, cudaStream_t s);
 int label_static_count(const float* labels, long long n, const int32_t* ids, int n_ids, int64_t* count, cudaStream_t s);
 }  // namespace nrw
+
+// ground-truth alignment check: first-hit splats at query pixels and per-observation reprojection errors (gtproj.cu)
+namespace nrw {
+long long first_hit_scratch_bytes(long long n_queries, long long map_pixels);
+int first_hit(const float* points, long long n_points, const double* views, const int32_t* boxes, int n_views,
+              const int32_t* q_view, const float* q_xy, long long n_q, int64_t* hit, int32_t* status, void* scratch,
+              long long scratch_bytes, cudaStream_t s);
+int obs_reproj_error(const double* X, const int32_t* view, const double* xy, long long n, const double* P, int n_views,
+                     double* err, double* uv, cudaStream_t s);
+}  // namespace nrw

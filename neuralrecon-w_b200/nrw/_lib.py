@@ -146,6 +146,10 @@ def lib():
     L.nrw_voxel_lookup.argtypes = [vp, vp, C.POINTER(i32), i32, vp, ll, vp, vp, vp]
     L.nrw_view_roi_count.argtypes = [vp, vp, i32, ll, C.POINTER(f32), f32, vp, vp]
     L.nrw_label_static_count.argtypes = [vp, ll, C.POINTER(i32), i32, vp, vp]
+    L.nrw_first_hit_scratch_bytes.restype = ll
+    L.nrw_first_hit_scratch_bytes.argtypes = [ll, ll]
+    L.nrw_first_hit.argtypes = [vp, ll, C.POINTER(f64), C.POINTER(i32), i32, vp, vp, ll, vp, vp, vp, ll, vp]
+    L.nrw_obs_reproj_error.argtypes = [vp, vp, vp, ll, vp, i32, vp, vp, vp]
     L.nrw_gemm_test_scratch_bytes.restype = ll
     L.nrw_gemm_test_scratch_bytes.argtypes = [i32, i32, i32]
     L.nrw_gemm_test.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp]
@@ -171,7 +175,8 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_mesh_sample", "nrw_raster_scratch_bytes", "nrw_raster_depth", "nrw_reproject_scratch_bytes",
            "nrw_reproject_mark", "nrw_raygen_capacity", "nrw_raygen_scratch_bytes", "nrw_raygen_image",
            "nrw_depth_range_scratch_bytes", "nrw_depth_range", "nrw_voxel_cast", "nrw_voxel_lookup",
-           "nrw_view_roi_count", "nrw_label_static_count"]
+           "nrw_view_roi_count", "nrw_label_static_count", "nrw_first_hit_scratch_bytes", "nrw_first_hit",
+           "nrw_obs_reproj_error"]
 
 
 def check(status, what=""):

@@ -7,11 +7,12 @@ import numpy as np
 from ._lib import NrwError
 
 
-def read_points3d(path):
+def read_points3d(path, with_tracks=False):
     """points3D.bin (utils/colmap_utils.py::read_points3d_binary layout, little endian): per point u64 id, 3 f64 xyz,
     3 u8 rgb, f64 error, u64 track length, then track length (i32 image id, i32 point2D index) pairs.  Returns a dict of
     numpy arrays in file order: id uint64 [n], xyz float64 [n,3], rgb uint8 [n,3], error float64 [n], track_length
-    int64 [n]."""
+    int64 [n].  With with_tracks the tracks come too, as CSR arrays: the pairs of point r are rows
+    track_offsets[r] .. track_offsets[r+1] of track_image_id int32 and track_point2d_idx int32, in track order."""
     with open(path, "rb") as fh:
         data = fh.read()
     if len(data) < 8:
@@ -23,17 +24,27 @@ def read_points3d(path):
     rgb = np.empty((n, 3), np.uint8)
     err = np.empty(n, np.float64)
     tl = np.empty(n, np.int64)
+    starts = np.empty(n, np.int64)
     off = 8
     try:
         for i in range(n):
             r = rec.unpack_from(data, off)
             ids[i], xyz[i], rgb[i], err[i], tl[i] = r[0], r[1:4], r[4:7], r[7], r[8]
+            starts[i] = off + rec.size
             off += rec.size + 8 * r[8]
     except struct.error as e:
         raise NrwError(f"read_points3d: {path} is truncated") from e
     if off > len(data):
         raise NrwError(f"read_points3d: {path} is truncated")
-    return {"id": ids, "xyz": xyz, "rgb": rgb, "error": err, "track_length": tl}
+    out = {"id": ids, "xyz": xyz, "rgb": rgb, "error": err, "track_length": tl}
+    if with_tracks:
+        offsets = np.zeros(n + 1, np.int64)
+        np.cumsum(tl, out=offsets[1:])
+        pairs = np.empty((int(offsets[-1]), 2), np.int32)
+        for i in range(n):
+            pairs[offsets[i]:offsets[i + 1]] = np.frombuffer(data, "<i4", 2 * int(tl[i]), int(starts[i])).reshape(-1, 2)
+        out.update(track_offsets=offsets, track_image_id=pairs[:, 0].copy(), track_point2d_idx=pairs[:, 1].copy())
+    return out
 
 
 # model id -> (name, number of parameters), COLMAP's camera models
