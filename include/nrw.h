@@ -197,6 +197,13 @@ NRW_API int nrw_composite_backward(const nrw_render_cfg* cfg, const nrw_render_i
                                    const nrw_render_grads* g, const float* normals_ps, float* d_sdf,
                                    float* d_normals_ps, float* d_rgb, float* d_bg_alpha, float* d_bg_rgb,
                                    void* stream);
+/* the network half of nrw_render_backward with injected per-sample upstream gradients: d_sdf [R,S], d_normals [R,S,3],
+ * d_rgb [R,S,3], and when n_outside > 0 d_bg_alpha [R,T], d_bg_rgb [R,T,3] in sv_z_feed order (all required, none
+ * means zero).  Reuses the forward that nrw_render_forward left in the context under the generation-stamp and
+ * recompute rules of nrw_render_backward; grad_params is ACCUMULATED into, grad_a_emb [R,n_a] is written. */
+NRW_API int nrw_network_backward(nrw_ctx* ctx, const nrw_render_cfg* cfg, const nrw_render_io* io, const float* d_sdf,
+                                 const float* d_normals, const float* d_rgb, const float* d_bg_alpha,
+                                 const float* d_bg_rgb, float* grad_params, float* grad_a_emb, void* stream);
 
 /* ---- octree near/far (tools/prepare_data/generate_voxel.py:311-439) ---------------------- */
 /* octree bytes (breadth-first, one per non-leaf), prefix = exclusive popcount sum (#nodes entries),

@@ -240,6 +240,19 @@ int nrw_composite_backward(const nrw_render_cfg* cfg, const nrw_render_io* io, c
                             S(stream));
   NRW_GUARD_END
 }
+int nrw_network_backward(nrw_ctx* ctx, const nrw_render_cfg* cfg, const nrw_render_io* io, const float* d_sdf,
+                         const float* d_normals, const float* d_rgb, const float* d_bg_alpha, const float* d_bg_rgb,
+                         float* grad_params, float* grad_a_emb, void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx && cfg && io && grad_params && grad_a_emb, NRW_ERR_ARG, "network_backward: null argument");
+  NRW_CHECK(d_sdf && d_normals && d_rgb, NRW_ERR_ARG, "network_backward: null upstream gradient");
+  NRW_CHECK(cfg->n_outside <= 0 || (d_bg_alpha && d_bg_rgb), NRW_ERR_ARG,
+            "network_backward: n_outside=%d needs both background upstream gradients", cfg->n_outside);
+  if (cfg->R == 0) return NRW_OK;
+  return network_backward(*ctx, *cfg, *io, d_sdf, d_normals, d_rgb, d_bg_alpha, d_bg_rgb, grad_params, grad_a_emb,
+                          S(stream));
+  NRW_GUARD_END
+}
 
 int nrw_octree_near_far(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid_host, int level,
                         const float* rays_o, const float* rays_d, int R, const float scene_origin[3], float scale,

@@ -594,17 +594,20 @@ static ChunkWalk chunk_walk(int j, int n, int n_slots, bool cached) {
   return ChunkWalk{ci, ci < last ? ci : last, cached && (ci == n - 1 || ci < last)};
 }
 
-int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, const nrw_render_grads& g,
-                    cudaStream_t s) {
-  const int R = cfg.R, S = cfg.S, T = cfg.S + cfg.n_outside;
+static int backward_ready(const nrw_ctx& c, int R, int T) {
   NRW_CHECK(c.bound && c.packed_valid && c.with_bwd, NRW_ERR_STATE, "render_backward: workspace not bound for backward");
   NRW_CHECK(R <= c.max_rays && T <= c.max_T, NRW_ERR_WORKSPACE, "render: R=%d T=%d exceed bound workspace", R, T);
+  return NRW_OK;
+}
+
+int network_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, const float* d_sdf,
+                     const float* d_nrm, const float* d_rgb, const float* d_bga, const float* d_bgc, float* grad_params,
+                     float* grad_a_emb, cudaStream_t s) {
+  const int R = cfg.R, S = cfg.S, T = cfg.S + cfg.n_outside;
+  NRW_TRY(backward_ready(c, R, T));
   const bool bg = cfg.n_outside > 0;
   NRW_CUDA_OK(cudaMemsetAsync(c.gs, 0, (size_t)c.pm.grad_floats * 4, s));
-  NRW_CUDA_OK(cudaMemsetAsync(g.grad_a_emb, 0, (size_t)R * c.n_a * 4, s));
-  NRW_TRY(composite_backward(cfg, io, g, io.sv_sdf, io.gradients, io.sv_rgb, bg ? io.sv_bg_alpha : nullptr,
-                             bg ? io.sv_bg_rgb : nullptr, c.g_dsdf, c.g_dnrm, c.g_drgb, bg ? c.g_dbga : nullptr,
-                             bg ? c.g_dbgc : nullptr, g.grad_inv_s, s));
+  NRW_CUDA_OK(cudaMemsetAsync(grad_a_emb, 0, (size_t)R * c.n_a * 4, s));
   // do the slots still hold this render's forward?  Otherwise every chunk is recomputed (the generation stamp guards
   // against a second render_forward having overwritten the slots: ADVICE r1)
   const bool cached = c.fwd_cached && c.cached_R == R && c.cached_S == S && c.cached_T == T && c.cached_gen == cfg.reserved0;
@@ -619,8 +622,8 @@ int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& 
       if (!w.resident)
         NRW_TRY(nerf_chunk_forward(c, M, io.o + r0 * 3, io.d + r0 * 3, io.sv_z_feed + (long long)r0 * T,
                                    io.sample_dist + r0, nullptr, io.a_emb + (long long)r0 * c.n_a, T, T, s));
-      NRW_TRY(nerf_chunk_backward(c, M, c.g_dbga + (long long)r0 * T, c.g_dbgc + (long long)r0 * T * 3,
-                                  g.grad_a_emb + (long long)r0 * c.n_a, nr, T, s));
+      NRW_TRY(nerf_chunk_backward(c, M, d_bga + (long long)r0 * T, d_bgc + (long long)r0 * T * 3,
+                                  grad_a_emb + (long long)r0 * c.n_a, nr, T, s));
     }
   }
   const int rc = c.Mc / S, n = cdiv(R, rc);
@@ -635,14 +638,24 @@ int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& 
       NRW_TRY(sdf_chunk_forward(c, M, c.PTS, true, true, s));
       NRW_TRY(color_chunk_forward(c, M, c.PTS, io.d + r0 * 3, io.a_emb + (long long)r0 * c.n_a, S, s));
     }
-    NRW_TRY(color_chunk_backward(c, M, c.g_drgb + (long long)r0 * S * 3, c.g_dnrm + (long long)r0 * S * 3, S,
-                                 g.grad_a_emb + (long long)r0 * c.n_a, nr, s));
-    NRW_TRY(sdf_chunk_backward(c, M, c.PTS, c.g_dsdf + (long long)r0 * S, s));
+    NRW_TRY(color_chunk_backward(c, M, d_rgb + (long long)r0 * S * 3, d_nrm + (long long)r0 * S * 3, S,
+                                 grad_a_emb + (long long)r0 * c.n_a, nr, s));
+    NRW_TRY(sdf_chunk_backward(c, M, c.PTS, d_sdf + (long long)r0 * S, s));
   }
   c.fwd_cached = false;
   c.use_sdf_slot(0);
   c.use_nerf_slot(0);
-  return unpack_grads(c.pm, c.tab, c.params, c.packed, c.gs, g.grad_params, s);
+  return unpack_grads(c.pm, c.tab, c.params, c.packed, c.gs, grad_params, s);
+}
+
+int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, const nrw_render_grads& g,
+                    cudaStream_t s) {
+  NRW_TRY(backward_ready(c, cfg.R, cfg.S + cfg.n_outside));
+  const bool bg = cfg.n_outside > 0;
+  NRW_TRY(composite_backward(cfg, io, g, io.sv_sdf, io.gradients, io.sv_rgb, bg ? io.sv_bg_alpha : nullptr,
+                             bg ? io.sv_bg_rgb : nullptr, c.g_dsdf, c.g_dnrm, c.g_drgb, bg ? c.g_dbga : nullptr,
+                             bg ? c.g_dbgc : nullptr, g.grad_inv_s, s));
+  return network_backward(c, cfg, io, c.g_dsdf, c.g_dnrm, c.g_drgb, c.g_dbga, c.g_dbgc, g.grad_params, g.grad_a_emb, s);
 }
 
 }  // namespace nrw

@@ -123,5 +123,10 @@ int sample(nrw_ctx& c, const nrw_sampler_cfg& cfg, int R, const float* o, const 
 int render_forward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, cudaStream_t s);
 int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, const nrw_render_grads& g,
                     cudaStream_t s);
+// the part of render_backward after the compositing: parameter and appearance-code gradients of the three networks
+// from per-sample upstream gradients d_sdf [R,S], d_nrm [R,S,3], d_rgb [R,S,3], d_bga [R,T], d_bgc [R,T,3]
+int network_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, const float* d_sdf,
+                     const float* d_nrm, const float* d_rgb, const float* d_bga, const float* d_bgc, float* grad_params,
+                     float* grad_a_emb, cudaStream_t s);
 
 }  // namespace nrw

@@ -100,6 +100,7 @@ def lib():
     L.nrw_render_backward.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(RenderIO), C.POINTER(RenderGrads), vp]
     L.nrw_composite_forward.argtypes = [C.POINTER(RenderCfg), C.POINTER(RenderIO)] + [vp] * 7
     L.nrw_composite_backward.argtypes = [C.POINTER(RenderCfg), C.POINTER(RenderIO), C.POINTER(RenderGrads)] + [vp] * 7
+    L.nrw_network_backward.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(RenderIO)] + [vp] * 8
     L.nrw_octree_near_far.argtypes = [vp, vp, vp, i32, vp, vp, i32, C.POINTER(f32), f32, vp, vp, vp, vp, vp]
     L.nrw_octree_hits.argtypes = [vp, vp, vp, i32, vp, vp, i32, C.POINTER(f32), f32, vp, vp, vp, vp, vp]
     L.nrw_octree_build_scratch_bytes.restype = ll
@@ -165,7 +166,8 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_ctx_create", "nrw_ctx_destroy", "nrw_packed_bytes", "nrw_workspace_bytes", "nrw_ctx_bind",
            "nrw_pack_weights", "nrw_sdf_query", "nrw_neuconw_forward", "nrw_nerf_forward", "nrw_sample",
            "nrw_samples_per_ray", "nrw_upsample_round", "nrw_render_forward", "nrw_render_backward",
-           "nrw_composite_forward", "nrw_composite_backward", "nrw_octree_near_far", "nrw_octree_hits",
+           "nrw_composite_forward", "nrw_composite_backward", "nrw_network_backward", "nrw_octree_near_far",
+           "nrw_octree_hits",
            "nrw_gemm_test_scratch_bytes", "nrw_gemm_test", "nrw_gemm_pair_test", "nrw_launch_count", "nrw_debug_gemm_profile",
            "nrw_gemm_timing", "nrw_ctx_set_backward_planes", "nrw_octree_build_scratch_bytes", "nrw_octree_build",
            "nrw_grad_sumsq", "nrw_adam_clip_step", "nrw_boundary_samples", "nrw_compact_scratch_bytes", "nrw_raycache_gather",
