@@ -43,17 +43,21 @@ int sdf_fused_forward(const SdfFusedDesc& d, cudaStream_t stream);
 long long gemm_tc_launch_count();
 // output columns of one gemm_tc tile (the caller of a split-K GEMM sizes k_slices from the tile count)
 inline int gemm_tc_tile_n(int N) { return N <= 64 ? 64 : 128; }
-// One-plane weight gradients (MN-major, out_f32 += scale * A^T B and nothing else) with M >= 256 and N > 64 run 256 x 128
-// items that both consumer warpgroups share; every other GEMM runs 128-row items.
-inline bool gemm_tc_dw_coop(const GemmDesc& g) {
+// A pure weight gradient: MN-major, out_f32 += scale * A^T B into 8-byte aligned rows and nothing else.  gemm_tc runs it with
+// the fragment red.add epilogue (cooperative or paired schedule).
+inline bool gemm_tc_dw_only(const GemmDesc& g) {
   const Epi& e = g.epi;
-  return g.mn_major && g.n_planes == 1 && g.M >= 256 && g.N > 64 && e.atomic && e.out_f32 && e.ld_f32 % 2 == 0 &&
-         (reinterpret_cast<uintptr_t>(e.out_f32) & 7) == 0 && !e.bias && !e.rowvec && !e.out_pre && !e.colsum;
+  return g.mn_major && e.atomic && e.out_f32 && e.ld_f32 % 2 == 0 && (reinterpret_cast<uintptr_t>(e.out_f32) & 7) == 0 &&
+         e.act == ACT_NONE && !e.bias && !e.rowvec && !e.colvec && !e.aux_u.p && !e.aux_q && !e.aux_add && !e.aux_relu && !e.out_pre &&
+         !e.out2 && !e.out_pl.p && !e.n_planes && !e.colsum && !e.head_w && !e.head_partial;
 }
+// One-plane pure weight gradients with M >= 256 and N > 64 run 256 x 128 items that both consumer warpgroups share; every
+// other GEMM runs 128-row items.
+inline bool gemm_tc_dw_coop(const GemmDesc& g) { return gemm_tc_dw_only(g) && g.n_planes == 1 && g.M >= 256 && g.N > 64; }
 inline int gemm_tc_tile_m(const GemmDesc& g) { return gemm_tc_dw_coop(g) ? 256 : 128; }
 
 // A backward layer's data GEMM and its weight gradient, which read no output of each other: one launch runs both, so the
-// weight gradient's MMAs fill the tensor-core time the data tiles' epilogues leave idle (gemm_tc.cu, MN_PAIR).
+// weight gradient's MMAs fill the tensor-core time the data tiles' epilogues leave idle (gemm_tc.cu, Sched::PAIR).
 struct GemmPair {
   GemmDesc data;   // K-major, one plane, 128-column tiles, non-atomic epilogue of kind GENERIC, TANGENT, REVERSE or RELU_BWD
   GemmDesc dw;     // MN-major, one plane, N >= 128, out_f32 += scale * A^T B and nothing else; k_slices as given

@@ -17,21 +17,24 @@
 //   the next items) overlap the MMAs and the epilogues.  A stage has a single consuming warpgroup.
 // * the epilogue stages a warpgroup's accumulators (64 columns of one 64-row half per round) through shared memory into the
 //   line layout the chunk epilogues take (epilogue_tc.cuh / epilogue_fast.cuh: two 32-row x 16-column chunks per warp and round).
-// * mn_major=1 consumes both operands "transposed" straight from their natural row-major
+// * Each instantiation runs one schedule (Sched): K-major ping-pong (data GEMMs), MN-major ping-pong, cooperative weight
+//   gradients, or paired launches.  All four share one producer loop and one consumer loop over the CTA's item list (tc_item);
+//   a schedule only changes compile-time properties of them (operand layout, item kinds, which warpgroup owns an item).
+// * MN-major operands (Sched::MNMAJOR) are consumed "transposed" straight from their natural row-major
 //   [rows=K][cols=M|N] layout (MN-major wgmma descriptors) - used for weight gradients
 //   dW = dY^T X with split-K over the sample dimension and fp32 atomics in the epilogue.
-// * MN_COOP (one-plane weight gradients with M >= 256, gemm_tc_dw_coop): a work item is a 256 x 128 tile x K-slice that
+// * Sched::COOP (one-plane weight gradients with M >= 256, gemm_tc_dw_coop): a work item is a 256 x 128 tile x K-slice that
 //   both consumer warpgroups run at the same time, warpgroup wg on rows 128 wg .. +127 (two m64n128 halves), both reading
 //   the stage's one B tile.  Per 64-row k-block that moves 48 KB for 4.2 MFLOP instead of 32 KB for 2.1 MFLOP.  No turn
 //   barrier: each stage's empty barrier counts all 8 consumer warps.  The epilogue is one fp32 vector reduction
 //   (red.global.add.v2.f32) per accumulator pair straight from the fragment: no staging tile and no named barriers, while
 //   the producer already loads the next item's k-blocks.
-// * MN_PAIR (gemm_tc_pair): one launch runs a backward layer's data GEMM and its weight gradient together.  Work items are
+// * Sched::PAIR (gemm_tc_pair): one launch runs a backward layer's data GEMM and its weight gradient together.  Work items are
 //   the 128 x 128 tiles of the one-plane K-major data GEMM (epilogue kind EK) and 128 x 128 x K-slice items of the one-plane
 //   MN-major dW.  Both fill the same 32 KB stage, so ring, stage count and barriers are those of the ping-pong schedule; the
 //   item kind (warp-uniform) selects the tensor maps, the descriptors and the epilogue: data tiles take the staged epilogue,
-//   dW items the fragment red.add of MN_COOP.  The combined list is laid out in rounds of gridDim.x items (round j = the j-th
-//   item of every CTA, so warpgroup j & 1 runs it): data and dW rounds alternate while both remain, then the rest follow.
+//   dW items the fragment red.add of Sched::COOP.  The combined list is laid out in rounds of gridDim.x items (round j = the
+//   j-th item of every CTA, so warpgroup j & 1 runs it): data and dW rounds alternate while both remain, then the rest follow.
 //   So one warpgroup runs a data tile's epilogue while the other runs a dW item's main loop on the tensor cores.  A dW
 //   round numbers its items tile-minor over consecutive K-slices: the CTAs of a round share each slice's operand slabs in L2.
 //   K-slice rule (host, gemm_tc_pair_k_slices): 128 k-blocks of 64 samples per dW item.  At the tensor-core peak a k-block
@@ -64,8 +67,6 @@ static constexpr int EPI_COLS = 64;                    // columns per epilogue r
 static constexpr int EPI_WG_BYTES = 64 * EPI_COLS * 4; // one warpgroup's staging tile [64 rows][64 columns]
 static constexpr int CS_BYTES = 1024;                  // column-sum accumulators: 128 columns of the current n-tile per warpgroup
 static constexpr int BAR_TURN = 4;                     // named barriers 4 + wg: warpgroup wg's turn at the tensor cores
-static constexpr int MN_COOP = 2;                      // MN_MAJOR value of the cooperative 256-row weight-gradient schedule
-static constexpr int MN_PAIR = 3;                      // MN_MAJOR value of a paired data GEMM + weight-gradient launch
 static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 32 * N_CONSUMER_WARPS <= 65536, "register file");
 static constexpr int BAR_BYTES = 256;                  // 2 x MAX_STAGES mbarriers
 static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + 2 * EPI_WG_BYTES + CS_BYTES;
@@ -85,7 +86,7 @@ struct TcParams {
   int k_slices;
   int m_tiles, n_tiles;
   Epi epi;
-  // MN_PAIR: the weight gradient, out_f32[dw_M, dw_N] += dw_scale * A2^T B2 (one plane, MN-major, split into dw_k_slices)
+  // Sched::PAIR: the weight gradient, out_f32[dw_M, dw_N] += dw_scale * A2^T B2 (one plane, MN-major, split into dw_k_slices)
   CUtensorMap tmA2, tmB2;
   int dw_M, dw_N, dw_K, dw_k_slices, dw_m_tiles, dw_n_tiles;
   float* dw_out;
@@ -94,8 +95,8 @@ struct TcParams {
   // optional cycle attribution (debug): per CTA 16 counters
   //  [0] producer: waiting for a free stage   [5] kernel cycles
   //  first warp of consumer warpgroup wg, o = 8 wg: [1 + o] waiting for TMA data   [3 + o] waiting for its turn at the
-  //  tensor cores   [4 + o] epilogue   [6 + o] tiles (MN_COOP: both warpgroups count every non-empty item; MN_PAIR: data
-  //  tiles)   [7 + o] MN_PAIR: dW items
+  //  tensor cores   [4 + o] epilogue   [6 + o] tiles (Sched::COOP: both warpgroups count every non-empty item; Sched::PAIR:
+  //  data tiles)   [7 + o] Sched::PAIR: dW items
   unsigned long long* prof;
 };
 #define NRW_PROF_T0(cond) const long long _t0 = (cond) ? clock64() : 0
@@ -262,16 +263,34 @@ __device__ __forceinline__ void dw_reduce(const float (&acc)[2][BN / 2], float* 
     }
 }
 
-// One work item of a CTA: output tile origin, k-block range [kb0, kb1) (empty: kb1 <= kb0), and for MN_PAIR its kind.
+// Schedule of one gemm_tc_kernel instantiation (header comment): K-major or MN-major ping-pong, cooperative weight gradients,
+// or a paired data GEMM + weight-gradient launch.  The kernel reads it only through the properties below.
+enum class Sched { KMAJOR, MNMAJOR, COOP, PAIR };
+// tmA / tmB hold MN-major planes; otherwise K-major ones
+constexpr bool mn_operands(Sched s) { return s == Sched::MNMAJOR || s == Sched::COOP; }
+// both consumer warpgroups run every item, warpgroup wg on its rows 128 wg .. +127: no turn barrier, and a stage's empty
+// barrier counts all 8 consumer warps
+constexpr bool shared_items(Sched s) { return s == Sched::COOP; }
+constexpr int item_rows(Sched s) { return shared_items(s) ? 2 * BM : BM; }
+// item kinds: data tiles (staged epilogue) and weight-gradient items (one MN-major plane, fragment red.add epilogue)
+constexpr bool data_items(Sched s) { return s != Sched::COOP; }
+constexpr bool dw_items(Sched s) { return s == Sched::COOP || s == Sched::PAIR; }
+// both kinds in one launch: the weight gradient's operands are tmA2 / tmB2, its output the dw_* fields
+constexpr bool paired(Sched s) { return data_items(s) && dw_items(s); }
+
+// operand layout of an item's k-blocks: K-major planes, MN-major planes, or one MN-major weight-gradient plane
+enum class Ops { K, MN, DW };
+
+// One work item of a CTA: output tile origin, k-block range [kb0, kb1) (empty: kb1 <= kb0), and its kind.
 struct TcItem { int m0, n0, kb0, kb1; bool dw; };
 
-// item j of this CTA.  Plain launches: item blockIdx.x + j gridDim.x of the slice-minor list.  MN_PAIR: round j (see the
-// header comment); positions past the end of a kind's last round are empty items.
-template <int BN, int TM, bool PAIR>
+// item j of this CTA.  Plain launches: item blockIdx.x + j gridDim.x of the slice-minor list.  Paired launches: round j
+// (see the header comment); positions past the end of a kind's last round are empty items.
+template <int BN, Sched S>
 __device__ __forceinline__ TcItem tc_item(const TcParams& p, int j, int kb_total, int kb_per) {
   TcItem it;
-  it.dw = false;
-  if constexpr (PAIR) {
+  it.dw = !data_items(S);
+  if constexpr (paired(S)) {
     const int G = gridDim.x;
     const int n_data = p.m_tiles * p.n_tiles, dw_tiles = p.dw_m_tiles * p.dw_n_tiles, n_dw = dw_tiles * p.dw_k_slices;
     const int rd = (n_data + G - 1) / G, rw = (n_dw + G - 1) / G, ri = min(rd, rw);
@@ -293,7 +312,7 @@ __device__ __forceinline__ TcItem tc_item(const TcParams& p, int j, int kb_total
   const int item = blockIdx.x + j * gridDim.x;
   const int ks = item % p.k_slices;
   const int t = item / p.k_slices;
-  it.n0 = (t % p.n_tiles) * BN; it.m0 = (t / p.n_tiles) * TM;
+  it.n0 = (t % p.n_tiles) * BN; it.m0 = (t / p.n_tiles) * item_rows(S);
   it.kb0 = ks * kb_per; it.kb1 = min(kb_total, it.kb0 + kb_per);
   return it;
 }
@@ -302,18 +321,13 @@ __device__ __forceinline__ TcItem tc_item(const TcParams& p, int j, int kb_total
 //   n_planes==1: (0,0); ==2: (0,1),(1,0),(0,0); ==3: (0,2),(2,0),(1,1),(0,1),(1,0),(0,0)
 // With q = n_products-1-p (q=0 is (hi,hi)): a_plane = nibble q of 0x021010, b_plane = nibble q of 0x201100.
 
-// EK: compile-time epilogue kind (epilogue_fast.cuh); MN-major launches use EK_GENERIC.  MN_MAJOR: 0 K-major, 1 MN-major
-// ping-pong, MN_COOP MN-major with 256-row items shared by both warpgroups, MN_PAIR K-major data tiles (kind EK) and
-// MN-major weight-gradient items in one ping-pong launch.
-template <int BN, int MN_MAJOR, int EK>
+// EK: compile-time epilogue kind of the data tiles (epilogue_fast.cuh); MN-major launches use EK_GENERIC.  S: the schedule.
+template <int BN, Sched S, int EK>
 __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
   static_assert(BN == 64 || BN == 128, "wgmma tile width");
-  constexpr bool COOP = MN_MAJOR == MN_COOP;
-  constexpr bool PAIR = MN_MAJOR == MN_PAIR;
-  constexpr int TR = MN_MAJOR == 1 ? 1 : 0;     // transpose flag of the (data) wgmma operands
-  static_assert(!COOP || (BN == 128 && EK == EK_GENERIC), "the cooperative schedule is the 256 x 128 weight-gradient tile");
-  static_assert(!PAIR || BN == 128, "paired launches run 128 x 128 items of both kinds");
-  constexpr int TM = COOP ? 2 * BM : BM;        // rows of a work item
+  static_assert(data_items(S) || (BN == 128 && EK == EK_GENERIC), "the cooperative schedule is the 256 x 128 weight-gradient tile");
+  static_assert(!paired(S) || BN == 128, "paired launches run 128 x 128 items of both kinds");
+  constexpr int TM = item_rows(S);              // rows of a work item
   constexpr int A_TILE = TM * BK * 2;
   constexpr int B_TILE = BN * BK * 2;
   constexpr int WG_A = 64 * BK * 2;           // one 64-row half of the A tile (K-major: 64 rows; MN-major: one 64-wide slab)
@@ -337,13 +351,13 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       tma_prefetch_desc(&p.tmA[i]);
       tma_prefetch_desc(&p.tmB[i]);
     }
-    if (PAIR) {
+    if (paired(S)) {
       tma_prefetch_desc(&p.tmA2);
       tma_prefetch_desc(&p.tmB2);
     }
     for (int i = 0; i < MAX_STAGES; ++i) {
       mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, COOP ? 8 : 4);   // the four warps of the stage's consuming warpgroup (COOP: both)
+      mbar_init(bar_empty + 8 * i, shared_items(S) ? 8 : 4);   // the four warps of the stage's consuming warpgroup (or both)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -356,8 +370,8 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
   const int kb_per = (kb_total + p.k_slices - 1) / p.k_slices;
   const int n_items = p.m_tiles * p.n_tiles * p.k_slices;
   const int n_prod = (P == 1) ? 1 : (P == 2 ? 3 : 6);
-  int n_j;   // items of this CTA (MN_PAIR: rounds, empty items included)
-  if constexpr (PAIR) {
+  int n_j;   // items of this CTA (paired: rounds, empty items included)
+  if constexpr (paired(S)) {
     const int G = gridDim.x, n_dw = p.dw_m_tiles * p.dw_n_tiles * p.dw_k_slices;
     n_j = (n_items + G - 1) / G + (n_dw + G - 1) / G;
   } else {
@@ -371,7 +385,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       int s = 0;
       uint32_t ph = 0;
       for (int j = 0; j < n_j; ++j) {
-        const TcItem it = tc_item<BN, TM, PAIR>(p, j, kb_total, kb_per);
+        const TcItem it = tc_item<BN, S>(p, j, kb_total, kb_per);
         const int n0 = it.n0, m0 = it.m0;
         for (int kb = it.kb0; kb < it.kb1; ++kb) {
           {
@@ -382,14 +396,14 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
           mbar_arrive_expect_tx(bar_full + 8 * s, stage_bytes);
           const uint32_t sa = smem_u32(smem + s * stage_bytes);
           const uint32_t sb = sa + P * A_TILE;
-          if (PAIR && it.dw) {                         // MN-major weight-gradient k-block: two 64-wide slabs of each operand
+          if (paired(S) && it.dw) {                    // MN-major weight-gradient k-block: two 64-wide slabs of each operand
 #pragma unroll
             for (int sl = 0; sl < 2; ++sl) {
               tma_load_2d(sa + sl * (64 * BK * 2), &p.tmA2, bar_full + 8 * s, m0 + 64 * sl, kb * BK);
               tma_load_2d(sb + sl * (64 * BK * 2), &p.tmB2, bar_full + 8 * s, n0 + 64 * sl, kb * BK);
             }
           } else for (int pl = 0; pl < P; ++pl) {
-            if (MN_MAJOR == 0 || PAIR) {
+            if (!mn_operands(S)) {
               tma_load_2d(sa + pl * A_TILE, &p.tmA[pl], bar_full + 8 * s, kb * BK, m0);
               tma_load_2d(sb + pl * B_TILE, &p.tmB[pl], bar_full + 8 * s, kb * BK, n0);
             } else {
@@ -407,84 +421,13 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
         }
       }
     }
-  } else if constexpr (COOP) {
-    // ===================== consumers: both warpgroups on every item, warpgroup wg on rows 128 wg .. +127 =====================
-    setmaxnreg_inc<CONSUMER_REGS>();
-    const int wg = warp >> 2, wi = warp & 3;
-    const uint32_t smem0 = smem_u32(smem);
-    const uint64_t desc_hi = make_gdesc(0, 64 * BK * 2, 1024);   // MN-major: LBO = stride between 64-wide slabs, SBO = 8 k-rows
-    constexpr uint32_t KSTEP = 16 * 128;                          // bytes per wgmma K=16
-    const bool prof = p.prof != nullptr && wi == 0 && lane == 0;
-    const int po = 8 * wg;
-    const int n_lim = min(p.N, p.epi.n_store);
-    int s = 0;
-    uint32_t ph = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int ks = item % p.k_slices;
-      const int t = item / p.k_slices;
-      const int n0 = (t % p.n_tiles) * BN, m0 = (t / p.n_tiles) * TM;
-      const int kb0 = ks * kb_per, kb1 = min(kb_total, kb0 + kb_per);
-      float acc[2][BN / 2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.0f;
-      int prev_s = -1;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        {
-          NRW_PROF_T0(prof);
-          mbar_wait(bar_full + 8 * s, ph);
-          NRW_PROF_ADD(prof, 1 + po);
-        }
-        const uint32_t sa = smem0 + s * stage_bytes;
-        const uint32_t sb = smem0 + s * stage_bytes + P * A_TILE;
-        wgmma_fence();
-        for (int pr = 0; pr < n_prod; ++pr) {
-          const int q = 4 * (n_prod - 1 - pr);
-          const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
-          const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE + 2 * wg * WG_A) & 0x3FFFFu) >> 4);
-          const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)                  // 64-wide A slab 2 wg + h
-              wgmma_bf16<BN, 1, 1>(acc[h], da + ((h * WG_A + k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
-        }
-        wgmma_commit();
-        acc_fence(acc[0]);
-        acc_fence(acc[1]);
-        if (prev_s >= 0) {                                // the previous stage's MMAs have completed: hand it back
-          wgmma_wait<1>();
-          acc_fence(acc[0]);
-          acc_fence(acc[1]);
-          if (lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
-        }
-        prev_s = s;
-        if (++s == stages) { s = 0; ph ^= 1; }
-      }
-      wgmma_wait<0>();
-      acc_fence(acc[0]);
-      acc_fence(acc[1]);
-      if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
-      if (kb1 <= kb0) continue;                           // an empty K-slice stores nothing
-      NRW_PROF_T0(prof);
-      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + 6 + po], 1ull);
-      dw_reduce<BN>(acc, p.epi.out_f32, p.epi.ld_f32, p.epi.scale, m0 + 128 * wg, n0, p.M, n_lim, wi, lane);
-      NRW_PROF_ADD(prof, 4 + po);
-    }
   } else {
-    // ===================== consumers: ping-pong warpgroups, each the MMAs and then the epilogue of its own items =====================
+    // ===================== consumers: each warpgroup runs the MMAs and then the epilogue of the items it owns =====================
     setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2, wi = warp & 3;
     const uint32_t smem0 = smem_u32(smem);
-    // K-major: SBO = 8 rows * 128 B; MN-major: LBO = stride between 64-wide MN slabs, SBO = 8 k-rows
-    constexpr uint32_t LBO = TR ? (64 * BK * 2) : 16;
-    constexpr uint32_t SBO = 1024;
-    constexpr uint32_t KSTEP = TR ? (16 * 128) : 32;         // bytes per wgmma K=16
-    constexpr uint32_t KSTEP_DW = 16 * 128;                  // MN_PAIR weight-gradient items (MN-major)
-    const uint64_t desc_hi = make_gdesc(0, LBO, SBO);         // everything but the start address
     float* stage_tile = epi_buf + wg * (EPI_WG_BYTES / 4);
-    const bool use_cs = p.epi.colsum != nullptr && !p.epi.atomic;
+    const bool use_cs = data_items(S) && p.epi.colsum != nullptr && !p.epi.atomic;
     float* cs_wg = cs_buf + 128 * wg;                        // this warpgroup's column-sum accumulator
     const int ctid = threadIdx.x & 127;
     const bool prof = p.prof != nullptr && wi == 0 && lane == 0;
@@ -492,12 +435,12 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
     int cs_n0 = -1;   // n-tile the column-sum accumulator currently holds
     int s = 0;        // ring position (stage, phase) of the next k-block, over every item of the CTA
     uint32_t ph = 0;
-    // item j of the CTA: items of both warpgroups are walked so that the ring position stays in step with the producer
+    // item j of the CTA: every item is walked, owned or not, so that the ring position stays in step with the producer
     for (int j = 0; j < n_j; ++j) {
-      const TcItem it = tc_item<BN, BM, PAIR>(p, j, kb_total, kb_per);
+      const TcItem it = tc_item<BN, S>(p, j, kb_total, kb_per);
       const int n0 = it.n0, m0 = it.m0, kb0 = it.kb0, kb1 = it.kb1;
-      const bool dw = PAIR && it.dw;                         // warp-uniform: a weight-gradient item of a paired launch
-      if ((j & 1) != wg) {                                   // the other warpgroup's item: skip its stages
+      const bool dw = it.dw;                                 // warp-uniform; compile-time unless paired
+      if (!shared_items(S) && (j & 1) != wg) {               // the other warpgroup's item: skip its stages
         for (int kb = kb0; kb < kb1; ++kb)
           if (++s == stages) { s = 0; ph ^= 1; }
         continue;
@@ -506,7 +449,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
         if (cs_n0 >= 0) colsum_flush(cs_wg, p.epi.colsum, cs_n0, min(min(p.N, p.epi.n_store) - cs_n0, BN), ctid, 128, 2 + wg);
         cs_n0 = n0;
       }
-      float acc[2][BN / 2];                                  // rows 0-63 and 64-127 of the tile
+      float acc[2][BN / 2];                                  // rows 0-63 and 64-127 of the warpgroup's 128
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -514,16 +457,21 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
       // Wait for this warpgroup's turn: the other one has issued every MMA of item j-1.  Besides keeping the tensor cores
       // with one warpgroup at a time, this is what makes the parity waits on the shared ring safe: every full-barrier
       // phase before this item's k-blocks has completed, so a stage cannot be seen one phase early.
-      if (j > 0) {
+      if (!shared_items(S) && j > 0) {
         NRW_PROF_T0(prof);
         named_bar_sync(BAR_TURN + wg, 256);
         NRW_PROF_ADD(prof, 3 + po);
       }
-      // The main loop, instantiated once per item kind (DW: a weight-gradient item of a paired launch, MN-major operands).
-      // Each kind's wgmma sequence, from the first fence to the final wait, lies on one path: wgmma variants that share
+      // One item's k-blocks, from the first wgmma fence to the release of the last stage, for operand layout L: K-major
+      // planes, MN-major planes, or one MN-major weight-gradient plane (Ops::DW, whose A slabs start at a_off).  Each item
+      // kind's wgmma sequence lies on one path, its own instantiation of this lambda: wgmma variants that share
       // accumulators under a per-k-block branch would make ptxas serialise every wgmma of the kernel.
-      auto main_loop = [&](auto kind) {
-        constexpr bool DW = decltype(kind)::value;
+      auto mma_item = [&](auto layout, uint32_t a_off) {
+        constexpr Ops L = decltype(layout)::value;
+        constexpr int TR = L == Ops::K ? 0 : 1;                // transpose flag of both wgmma operands
+        constexpr uint32_t KSTEP = TR ? (16 * 128) : 32;      // bytes per wgmma K=16
+        // K-major: SBO = 8 rows * 128 B; MN-major: LBO = stride between 64-wide MN slabs, SBO = 8 k-rows
+        const uint64_t desc_hi = make_gdesc(0, TR ? (64 * BK * 2) : 16, 1024);   // everything but the start address
         int prev_s = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
           {
@@ -534,32 +482,21 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
           const uint32_t sa = smem0 + s * stage_bytes;
           const uint32_t sb = smem0 + s * stage_bytes + P * A_TILE;
           wgmma_fence();
-          if constexpr (DW) {                            // one plane, both operands MN-major
-            const uint64_t desc_dw = make_gdesc(0, 64 * BK * 2, SBO);
-            const uint64_t da = desc_dw | (uint64_t)((sa & 0x3FFFFu) >> 4);
-            const uint64_t db = desc_dw | (uint64_t)((sb & 0x3FFFFu) >> 4);
+          for (int pr = 0; pr < (L == Ops::DW ? 1 : n_prod); ++pr) {
+            const int q = 4 * (n_prod - 1 - pr);             // product order of product_planes(), packed lookup
+            const uint32_t pa = L == Ops::DW ? 0 : (0x021010u >> q) & 0xFu, pb = L == Ops::DW ? 0 : (0x201100u >> q) & 0xFu;
+            const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE + a_off) & 0x3FFFFu) >> 4);
+            const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
 #pragma unroll
             for (int k = 0; k < BK / 16; ++k)
 #pragma unroll
-              for (int h = 0; h < 2; ++h)
-                wgmma_bf16<BN, 1, 1>(acc[h], da + ((h * WG_A + k * KSTEP_DW) >> 4), db + ((k * KSTEP_DW) >> 4), 1u);
-          } else {
-            for (int pr = 0; pr < n_prod; ++pr) {
-              const int q = 4 * (n_prod - 1 - pr);         // product order of product_planes(), packed lookup
-              const uint32_t pa = (0x021010u >> q) & 0xFu, pb = (0x201100u >> q) & 0xFu;
-              const uint64_t da = desc_hi | (uint64_t)(((sa + pa * A_TILE) & 0x3FFFFu) >> 4);
-              const uint64_t db = desc_hi | (uint64_t)(((sb + pb * B_TILE) & 0x3FFFFu) >> 4);
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)                // 64-row half h: K-major rows at +8 KB, or the second MN-major slab
-                  wgmma_bf16<BN, TR, TR>(acc[h], da + ((h * WG_A + k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
-            }
+              for (int h = 0; h < 2; ++h)                    // 64-row half h: K-major rows at +8 KB, or the next MN-major slab
+                wgmma_bf16<BN, TR, TR>(acc[h], da + ((h * WG_A + k * KSTEP) >> 4), db + ((k * KSTEP) >> 4), 1u);
           }
           wgmma_commit();
           acc_fence(acc[0]);
           acc_fence(acc[1]);
-          if (prev_s >= 0) {                              // the previous stage's MMAs have completed: hand it back
+          if (prev_s >= 0) {                                  // the previous stage's MMAs have completed: hand it back
             wgmma_wait<1>();
             acc_fence(acc[0]);
             acc_fence(acc[1]);
@@ -569,20 +506,21 @@ __global__ void __launch_bounds__(N_THREADS, 1) gemm_tc_kernel(const __grid_cons
           if (++s == stages) { s = 0; ph ^= 1; }
         }
         // every MMA of this item is issued: the other warpgroup's main loop may start (if the CTA has an item j+1)
-        if (j + 1 < n_j) named_bar_arrive(BAR_TURN + (wg ^ 1), 256);
+        if (!shared_items(S) && j + 1 < n_j) named_bar_arrive(BAR_TURN + (wg ^ 1), 256);
         wgmma_wait<0>();
         acc_fence(acc[0]);
         acc_fence(acc[1]);
         if (prev_s >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_s);
       };
-      if (dw) main_loop(std::true_type{});
-      else main_loop(std::false_type{});
+      if (dw) mma_item(std::integral_constant<Ops, Ops::DW>{}, shared_items(S) ? 2 * wg * WG_A : 0);   // shared: A slabs 2 wg, 2 wg + 1
+      else mma_item(std::integral_constant<Ops, mn_operands(S) ? Ops::MN : Ops::K>{}, 0);
       // (an empty k-slice accumulates nothing and stores nothing)
       if (kb1 <= kb0) continue;
       NRW_PROF_T0(prof);
-      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + (dw ? 7 : 6) + po], 1ull);
+      if (prof) atomicAdd(&p.prof[blockIdx.x * 16 + (paired(S) && dw ? 7 : 6) + po], 1ull);
       if (dw) {
-        dw_reduce<BN>(acc, p.dw_out, p.dw_ld, p.dw_scale, m0, n0, p.dw_M, p.dw_N, wi, lane);
+        if (paired(S)) dw_reduce<BN>(acc, p.dw_out, p.dw_ld, p.dw_scale, m0, n0, p.dw_M, p.dw_N, wi, lane);
+        else dw_reduce<BN>(acc, p.epi.out_f32, p.epi.ld_f32, p.epi.scale, m0 + 128 * wg, n0, p.M, min(p.N, p.epi.n_store), wi, lane);
         NRW_PROF_ADD(prof, 4 + po);
         continue;
       }
@@ -731,39 +669,40 @@ static int current_device() {
   return (dev >= 0 && dev < MAX_DEV) ? dev : 0;
 }
 
-// every tcgen05 GEMM goes through here.  NRW_PDL (default 1; 0 = plain launches): programmatic dependent launch (see pdl_wait); consecutive GEMMs of a layer
-// chain then overlap their prologues with the predecessor's tail.  Other kernels of the stream are launched normally and
-// serialise as usual.
-template <typename Kernel>
-static cudaError_t launch_gemm(Kernel kernel, int grid, int block, cudaStream_t stream, const TcParams& p) {
-  static const int pdl = getenv("NRW_PDL") ? atoi(getenv("NRW_PDL")) : 1;
+// Every tensor-core kernel goes through here: grid = min(items, SMs) persistent CTAs, launched with programmatic dependent
+// launch (see pdl_wait), so consecutive GEMMs of a layer chain overlap their prologues with the predecessor's tail.  Other
+// kernels of the stream are launched normally and serialise as usual.
+template <auto Kernel, typename Params>
+static int launch_tc(const Params& p, int items, int threads, int smem_bytes, cudaStream_t stream) {
+  static bool attr_set[MAX_DEV] = {false};
+  static int n_sm[MAX_DEV] = {0};
+  const int dev = current_device();
+  if (!attr_set[dev]) {
+    NRW_CUDA_OK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    attr_set[dev] = true;
+  }
+  if (!n_sm[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm[dev], cudaDevAttrMultiProcessorCount, dev));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid, 1, 1);
-  cfg.blockDim = dim3(block, 1, 1);
-  cfg.dynamicSmemBytes = SMEM_BYTES;
+  cfg.gridDim = dim3(std::min(items, n_sm[dev]), 1, 1);
+  cfg.blockDim = dim3(threads, 1, 1);
+  cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, p);
-}
-
-template <int BN, int MN, int EK>
-static int launch(const TcParams& p, int n_sm, int dev, cudaStream_t stream) {
-  static bool attr_set[MAX_DEV] = {false};
-  if (!attr_set[dev]) {
-    NRW_CUDA_OK((cudaFuncSetAttribute(gemm_tc_kernel<BN, MN, EK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)));
-    attr_set[dev] = true;
-  }
-  const int items = p.m_tiles * p.n_tiles * p.k_slices + (MN == MN_PAIR ? p.dw_m_tiles * p.dw_n_tiles * p.dw_k_slices : 0);
-  const int grid = items < n_sm ? items : n_sm;
-  NRW_CUDA_OK((launch_gemm(gemm_tc_kernel<BN, MN, EK>, grid, N_THREADS, stream, p)));
+  cfg.numAttrs = 1;
+  NRW_CUDA_OK(cudaLaunchKernelEx(&cfg, Kernel, p));
   NRW_LAUNCH_OK();
   ++g_tc_launches;
   return NRW_OK;
+}
+
+template <int BN, Sched S, int EK>
+static int launch(const TcParams& p, cudaStream_t stream) {
+  const int items = p.m_tiles * p.n_tiles * p.k_slices + (paired(S) ? p.dw_m_tiles * p.dw_n_tiles * p.dw_k_slices : 0);
+  return launch_tc<gemm_tc_kernel<BN, S, EK>>(p, items, N_THREADS, SMEM_BYTES, stream);
 }
 
 static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream);
@@ -775,6 +714,7 @@ struct TimedLaunch {
   cudaEvent_t e0, e1; double flops; double mma_flops; int M, N, K, P, mn, ks; unsigned epi; double bytes;
   int M2 = 0, N2 = 0, K2 = 0, ks2 = 0;
 };
+static constexpr int TIMED_MN_PAIR = 3;   // TimedLaunch::mn (the dump's mn_major column) of a paired launch
 static std::vector<TimedLaunch> g_timed;
 static std::vector<cudaEvent_t> g_event_pool;
 static bool g_timing_on = false;
@@ -798,7 +738,7 @@ int gemm_tc_timing_read(double* ms, double* flops, double* mma_flops, long long*
     NRW_CUDA_OK(cudaEventElapsedTime(&dt, L.e0, L.e1));
     t += dt; f += L.flops; mf += L.mma_flops; by += L.bytes;
     g_event_pool.push_back(L.e0); g_event_pool.push_back(L.e1);
-    if (dump && L.mn == MN_PAIR)
+    if (dump && L.mn == TIMED_MN_PAIR)
       fprintf(dump, "%d,%d,%d,%d,%d,%d,%u,%.0f,%.4f,%d,%d,%d,%d\n", L.M, L.N, L.K, L.P, L.mn, L.ks, L.epi, L.bytes, dt, L.M2, L.N2,
               L.K2, L.ks2);
     else if (dump) fprintf(dump, "%d,%d,%d,%d,%d,%d,%u,%.0f,%.4f\n", L.M, L.N, L.K, L.P, L.mn, L.ks, L.epi, L.bytes, dt);
@@ -808,6 +748,19 @@ int gemm_tc_timing_read(double* ms, double* flops, double* mma_flops, long long*
   if (bytes) *bytes = by;
   g_timed.clear();
   return NRW_OK;
+}
+
+// Runs launch(); with timing on, between two events on `stream`, recorded with the TimedLaunch that describe() returns.
+template <typename Describe, typename Launch>
+static int timed(cudaStream_t stream, Describe describe, Launch launch) {
+  if (!g_timing_on) return launch();
+  TimedLaunch L = describe();
+  L.e0 = get_event(); L.e1 = get_event();
+  NRW_CUDA_OK(cudaEventRecord(L.e0, stream));
+  const int rc = launch();
+  NRW_CUDA_OK(cudaEventRecord(L.e1, stream));
+  g_timed.push_back(L);
+  return rc;
 }
 
 // adds g's algorithmic FLOP, MMA FLOP and bytes to L
@@ -821,9 +774,8 @@ static void account(const GemmDesc& g, TimedLaunch& L) {
              mn * (4.0 * (e.out_f32 ? 1 : 0) + e.out2.elem_bytes() + q_bytes + e.aux_add.elem_bytes() + 2.0 * e.n_planes +
                    (e.aux_relu ? 2.0 : 0.0) + (e.aux_u.p ? 2.0 * e.aux_u_planes : 0.0));
 }
-static TimedLaunch timed_launch(const GemmDesc& g) {
+static TimedLaunch describe(const GemmDesc& g) {
   TimedLaunch L;
-  L.e0 = get_event(); L.e1 = get_event();
   L.flops = L.mma_flops = L.bytes = 0.0;
   account(g, L);
   L.M = g.M; L.N = g.N; L.K = g.K; L.P = g.n_planes; L.mn = g.mn_major; L.ks = g.k_slices;
@@ -835,35 +787,37 @@ static TimedLaunch timed_launch(const GemmDesc& g) {
 }
 
 int gemm_tc(const GemmDesc& g, cudaStream_t stream) {
-  if (!g_timing_on) return gemm_tc_impl(g, stream);
-  TimedLaunch L = timed_launch(g);
-  NRW_CUDA_OK(cudaEventRecord(L.e0, stream));
-  const int rc = gemm_tc_impl(g, stream);
-  NRW_CUDA_OK(cudaEventRecord(L.e1, stream));
-  g_timed.push_back(L);
-  return rc;
+  return timed(stream, [&] { return describe(g); }, [&] { return gemm_tc_impl(g, stream); });
 }
 
-static int sm_count(int dev, int& n_sm) {
-  static int n_sm_dev[MAX_DEV] = {0};
-  if (!n_sm_dev[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm_dev[dev], cudaDevAttrMultiProcessorCount, dev));
-  n_sm = n_sm_dev[dev];
+// tensor maps of operand plane pl of g for tiles bn columns wide: K-major rows in boxes of BK x rows, or MN-major 64-wide
+// slabs of BK k-rows
+static int operand_maps(const GemmDesc& g, int pl, int bn, CUtensorMap* a, CUtensorMap* b) {
+  if (!g.mn_major) {
+    NRW_CHECK(g.K % BK == 0, NRW_ERR_ARG, "gemm_tc: K=%d must be a multiple of %d (pad the operand)", g.K, BK);
+    NRW_TRY(make_map(a, g.A.plane(pl), g.K, g.M, g.A.ld, BK, BM));
+    return make_map(b, g.B.plane(pl), g.K, g.N, g.B.ld, BK, bn);
+  }
+  NRW_TRY(make_map(a, g.A.plane(pl), g.M, g.K, g.A.ld, 64, BK));
+  return make_map(b, g.B.plane(pl), g.N, g.K, g.B.ld, 64, BK);
+}
+
+// launch parameters of g on items of item_rows x bn
+static int tc_params(const GemmDesc& g, int item_rows, int bn, TcParams& p) {
+  memset(&p, 0, sizeof(p));
+  p.M = g.M; p.N = g.N; p.K = g.K; p.n_planes = g.n_planes; p.k_slices = g.k_slices;
+  p.m_tiles = cdiv(g.M, item_rows); p.n_tiles = cdiv(g.N, bn);
+  p.epi = g.epi;
+  p.prof = g_prof_ptr;
+  for (int pl = 0; pl < g.n_planes; ++pl) NRW_TRY(operand_maps(g, pl, bn, &p.tmA[pl], &p.tmB[pl]));
   return NRW_OK;
-}
-
-// weight gradients that run as the fragment red.add epilogue: out_f32 += scale * A^T B and nothing else, 8-byte aligned rows
-static bool dw_only(const GemmDesc& g) {
-  const Epi& e = g.epi;
-  return g.mn_major && e.atomic && e.out_f32 && e.ld_f32 % 2 == 0 && (reinterpret_cast<uintptr_t>(e.out_f32) & 7) == 0 &&
-         e.act == ACT_NONE && !e.bias && !e.rowvec && !e.colvec && !e.aux_u.p && !e.aux_q && !e.aux_add && !e.aux_relu && !e.out_pre && !e.out2 &&
-         !e.out_pl.p && !e.n_planes && !e.colsum && !e.head_w && !e.head_partial;
 }
 
 bool gemm_tc_pair_ok(const GemmPair& pr) {
   const GemmDesc &d = pr.data, &w = pr.dw;
   const int ek = d.mn_major ? -1 : pick_epi_kind(d.epi);
   return d.n_planes == 1 && w.n_planes == 1 && d.k_slices == 1 && !d.epi.atomic && gemm_tc_tile_n(d.N) == 128 &&
-         (ek == EK_GENERIC || ek == EK_TANGENT || ek == EK_REVERSE || ek == EK_RELU_BWD) && w.N >= 128 && dw_only(w);
+         (ek == EK_GENERIC || ek == EK_TANGENT || ek == EK_REVERSE || ek == EK_RELU_BWD) && w.N >= 128 && gemm_tc_dw_only(w);
 }
 
 static int gemm_tc_pair_impl(const GemmPair& pr, cudaStream_t stream) {
@@ -871,86 +825,58 @@ static int gemm_tc_pair_impl(const GemmPair& pr, cudaStream_t stream) {
   NRW_CHECK(d.M > 0 && d.N > 0 && d.K > 0 && w.M > 0 && w.N > 0 && w.K > 0 && w.k_slices >= 1, NRW_ERR_ARG,
             "gemm_tc_pair: empty problem %d %d %d / %d %d %d", d.M, d.N, d.K, w.M, w.N, w.K);
   NRW_CHECK(gemm_tc_pair_ok(pr), NRW_ERR_ARG, "gemm_tc_pair: the two GEMMs cannot share a launch");
-  NRW_CHECK(d.K % BK == 0, NRW_ERR_ARG, "gemm_tc_pair: K=%d must be a multiple of %d (pad the operand)", d.K, BK);
-  const int dev = current_device();
-  int n_sm = 0;
-  NRW_TRY(sm_count(dev, n_sm));
   TcParams p;
-  memset(&p, 0, sizeof(p));
-  p.M = d.M; p.N = d.N; p.K = d.K; p.n_planes = 1; p.k_slices = 1;
-  p.m_tiles = cdiv(d.M, BM); p.n_tiles = cdiv(d.N, 128);
-  p.epi = d.epi;
-  p.prof = g_prof_ptr;
-  NRW_TRY(make_map(&p.tmA[0], d.A.plane(0), d.K, d.M, d.A.ld, BK, BM));
-  NRW_TRY(make_map(&p.tmB[0], d.B.plane(0), d.K, d.N, d.B.ld, BK, 128));
-  NRW_TRY(make_map(&p.tmA2, w.A.plane(0), w.M, w.K, w.A.ld, 64, BK));
-  NRW_TRY(make_map(&p.tmB2, w.B.plane(0), w.N, w.K, w.B.ld, 64, BK));
+  NRW_TRY(tc_params(d, BM, 128, p));
+  NRW_TRY(operand_maps(w, 0, 128, &p.tmA2, &p.tmB2));
   p.dw_M = w.M; p.dw_N = std::min(w.N, w.epi.n_store); p.dw_K = w.K; p.dw_k_slices = w.k_slices;
   p.dw_m_tiles = cdiv(w.M, BM); p.dw_n_tiles = cdiv(w.N, 128);
   p.dw_out = w.epi.out_f32; p.dw_ld = w.epi.ld_f32; p.dw_scale = w.epi.scale;
   switch (pick_epi_kind(d.epi)) {
-    case EK_TANGENT: return launch<128, MN_PAIR, EK_TANGENT>(p, n_sm, dev, stream);
-    case EK_REVERSE: return launch<128, MN_PAIR, EK_REVERSE>(p, n_sm, dev, stream);
-    case EK_RELU_BWD: return launch<128, MN_PAIR, EK_RELU_BWD>(p, n_sm, dev, stream);
-    default: return launch<128, MN_PAIR, EK_GENERIC>(p, n_sm, dev, stream);
+    case EK_TANGENT: return launch<128, Sched::PAIR, EK_TANGENT>(p, stream);
+    case EK_REVERSE: return launch<128, Sched::PAIR, EK_REVERSE>(p, stream);
+    case EK_RELU_BWD: return launch<128, Sched::PAIR, EK_RELU_BWD>(p, stream);
+    default: return launch<128, Sched::PAIR, EK_GENERIC>(p, stream);
   }
 }
 
 int gemm_tc_pair(const GemmPair& pr, cudaStream_t stream) {
-  if (!g_timing_on) return gemm_tc_pair_impl(pr, stream);
-  TimedLaunch L = timed_launch(pr.data);
-  account(pr.dw, L);
-  L.mn = MN_PAIR;
-  L.M2 = pr.dw.M; L.N2 = pr.dw.N; L.K2 = pr.dw.K; L.ks2 = pr.dw.k_slices;
-  NRW_CUDA_OK(cudaEventRecord(L.e0, stream));
-  const int rc = gemm_tc_pair_impl(pr, stream);
-  NRW_CUDA_OK(cudaEventRecord(L.e1, stream));
-  g_timed.push_back(L);
-  return rc;
+  return timed(
+      stream,
+      [&] {
+        TimedLaunch L = describe(pr.data);
+        account(pr.dw, L);
+        L.mn = TIMED_MN_PAIR;
+        L.M2 = pr.dw.M; L.N2 = pr.dw.N; L.K2 = pr.dw.K; L.ks2 = pr.dw.k_slices;
+        return L;
+      },
+      [&] { return gemm_tc_pair_impl(pr, stream); });
 }
 
 static int gemm_tc_impl(const GemmDesc& g, cudaStream_t stream) {
   NRW_CHECK(g.M > 0 && g.N > 0 && g.K > 0, NRW_ERR_ARG, "gemm_tc: empty problem %d %d %d", g.M, g.N, g.K);
   NRW_CHECK(g.n_planes >= 1 && g.n_planes <= 3, NRW_ERR_ARG, "gemm_tc: n_planes=%d", g.n_planes);
   NRW_CHECK(g.k_slices == 1 || g.epi.atomic, NRW_ERR_ARG, "gemm_tc: split-K needs an atomic epilogue");
-  const int dev = current_device();
-  int n_sm = 0;
-  NRW_TRY(sm_count(dev, n_sm));
   // 128 x 128 tiles (one warpgroup, two m64n128 halves): with two operand planes that is 64 KB per k-block and 3 TMA stages
   const int BN = gemm_tc_tile_n(g.N);
-  const bool coop = gemm_tc_dw_coop(g);
   TcParams p;
-  memset(&p, 0, sizeof(p));
-  p.M = g.M; p.N = g.N; p.K = g.K; p.n_planes = g.n_planes; p.k_slices = g.k_slices;
-  p.m_tiles = cdiv(g.M, gemm_tc_tile_m(g)); p.n_tiles = cdiv(g.N, BN);
-  p.epi = g.epi;
-  p.prof = g_prof_ptr;
-  for (int pl = 0; pl < g.n_planes; ++pl) {
-    if (!g.mn_major) {
-      NRW_CHECK(g.K % BK == 0, NRW_ERR_ARG, "gemm_tc: K=%d must be a multiple of %d (pad the operand)", g.K, BK);
-      NRW_TRY(make_map(&p.tmA[pl], g.A.plane(pl), g.K, g.M, g.A.ld, BK, BM));
-      NRW_TRY(make_map(&p.tmB[pl], g.B.plane(pl), g.K, g.N, g.B.ld, BK, BN));
-    } else {
-      NRW_TRY(make_map(&p.tmA[pl], g.A.plane(pl), g.M, g.K, g.A.ld, 64, BK));
-      NRW_TRY(make_map(&p.tmB[pl], g.B.plane(pl), g.N, g.K, g.B.ld, 64, BK));
-    }
-  }
+  NRW_TRY(tc_params(g, gemm_tc_tile_m(g), BN, p));
   const int ek = g.mn_major ? EK_GENERIC : pick_epi_kind(g.epi);
   NRW_CHECK(ek >= 0 && (ek != EK_FWD_HEAD || g.N == 512), NRW_ERR_ARG,
             "gemm_tc: the fused SDF-head epilogue needs N = 512, bias + softplus and no other output");
-  if (coop) return launch<128, MN_COOP, EK_GENERIC>(p, n_sm, dev, stream);
-  if (g.mn_major) return BN == 64 ? launch<64, 1, EK_GENERIC>(p, n_sm, dev, stream) : launch<128, 1, EK_GENERIC>(p, n_sm, dev, stream);
-  if (BN == 64) return launch<64, 0, EK_GENERIC>(p, n_sm, dev, stream);
+  if (gemm_tc_dw_coop(g)) return launch<128, Sched::COOP, EK_GENERIC>(p, stream);
+  if (g.mn_major)
+    return BN == 64 ? launch<64, Sched::MNMAJOR, EK_GENERIC>(p, stream) : launch<128, Sched::MNMAJOR, EK_GENERIC>(p, stream);
+  if (BN == 64) return launch<64, Sched::KMAJOR, EK_GENERIC>(p, stream);
   switch (ek) {
-    case EK_FWD_SOFTPLUS: return launch<128, 0, EK_FWD_SOFTPLUS>(p, n_sm, dev, stream);
-    case EK_FWD_RELU: return launch<128, 0, EK_FWD_RELU>(p, n_sm, dev, stream);
-    case EK_FWD_NONE: return launch<128, 0, EK_FWD_NONE>(p, n_sm, dev, stream);
-    case EK_FWD_HEAD: return launch<128, 0, EK_FWD_HEAD>(p, n_sm, dev, stream);
-    case EK_GATE_FWD: return launch<128, 0, EK_GATE_FWD>(p, n_sm, dev, stream);
-    case EK_TANGENT: return launch<128, 0, EK_TANGENT>(p, n_sm, dev, stream);
-    case EK_REVERSE: return launch<128, 0, EK_REVERSE>(p, n_sm, dev, stream);
-    case EK_RELU_BWD: return launch<128, 0, EK_RELU_BWD>(p, n_sm, dev, stream);
-    default: return launch<128, 0, EK_GENERIC>(p, n_sm, dev, stream);
+    case EK_FWD_SOFTPLUS: return launch<128, Sched::KMAJOR, EK_FWD_SOFTPLUS>(p, stream);
+    case EK_FWD_RELU: return launch<128, Sched::KMAJOR, EK_FWD_RELU>(p, stream);
+    case EK_FWD_NONE: return launch<128, Sched::KMAJOR, EK_FWD_NONE>(p, stream);
+    case EK_FWD_HEAD: return launch<128, Sched::KMAJOR, EK_FWD_HEAD>(p, stream);
+    case EK_GATE_FWD: return launch<128, Sched::KMAJOR, EK_GATE_FWD>(p, stream);
+    case EK_TANGENT: return launch<128, Sched::KMAJOR, EK_TANGENT>(p, stream);
+    case EK_REVERSE: return launch<128, Sched::KMAJOR, EK_REVERSE>(p, stream);
+    case EK_RELU_BWD: return launch<128, Sched::KMAJOR, EK_RELU_BWD>(p, stream);
+    default: return launch<128, Sched::KMAJOR, EK_GENERIC>(p, stream);
   }
 }
 
@@ -1193,45 +1119,15 @@ int sdf_fused_forward(const SdfFusedDesc& d, cudaStream_t stream) {
   }
   p.head_w = d.head_w; p.head_b = d.head_b; p.pts = d.pts; p.sdf = d.sdf; p.M = d.M;
   p.n_tiles = cdiv(d.M, FZ_ROWS);
-  static int n_sm_dev[MAX_DEV] = {0};
-  static bool attr_set[MAX_DEV] = {false};
-  const int dev = current_device();
-  if (!n_sm_dev[dev]) NRW_CUDA_OK(cudaDeviceGetAttribute(&n_sm_dev[dev], cudaDevAttrMultiProcessorCount, dev));
-  if (!attr_set[dev]) {
-    NRW_CUDA_OK(cudaFuncSetAttribute(sdf_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FZ_SMEM));
-    attr_set[dev] = true;
-  }
-  int grid = n_sm_dev[dev];
-  if (p.n_tiles < grid) grid = p.n_tiles;
-  static const int pdl = getenv("NRW_PDL") ? atoi(getenv("NRW_PDL")) : 1;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid, 1, 1);
-  cfg.blockDim = dim3(FZ_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = FZ_SMEM;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  TimedLaunch L;
-  if (g_timing_on) {   // bench.py roofline: this launch replaces the 8 per-layer GEMMs of a forward-only chunk
-    L.e0 = get_event(); L.e1 = get_event();
+  auto describe_fused = [&] {   // bench.py roofline: this launch replaces the 8 per-layer GEMMs of a forward-only chunk
+    TimedLaunch L;
     L.flops = 2.0 * d.M * 512.0 * (64.0 + 7.0 * 512.0);
     L.mma_flops = 3.0 * L.flops;
     L.M = d.M; L.N = 512; L.K = 64 + 7 * 512; L.P = 2; L.mn = 0; L.ks = 1; L.epi = 4096u;
     L.bytes = 16.0 * d.M;
-    NRW_CUDA_OK(cudaEventRecord(L.e0, stream));
-  }
-  NRW_CUDA_OK(cudaLaunchKernelEx(&cfg, sdf_fused_kernel, p));
-  if (g_timing_on) {
-    NRW_CUDA_OK(cudaEventRecord(L.e1, stream));
-    g_timed.push_back(L);
-  }
-  NRW_LAUNCH_OK();
-  ++g_tc_launches;
-  return NRW_OK;
+    return L;
+  };
+  return timed(stream, describe_fused, [&] { return launch_tc<sdf_fused_kernel>(p, p.n_tiles, FZ_THREADS, FZ_SMEM, stream); });
 }
 
 }  // namespace nrw

@@ -1,4 +1,4 @@
-"""GPU: paired backward launches (gemm_tc.cu, MN_PAIR).  A backward layer's data GEMM and its weight gradient run as one
+"""GPU: paired backward launches (gemm_tc.cu, Sched::PAIR).  A backward layer's data GEMM and its weight gradient run as one
 launch: 128 x 128 data tiles with their specialised epilogue and 128 x 128 x K-slice dW items with the fragment red.add.
 Through nrw_gemm_pair_test, every data output of the paired launch is bit-identical to the same GEMM launched alone (the
 tile MMAs and the epilogue are unchanged), column sums agree to fp32 reordering, and dW agrees with an fp64 product of the

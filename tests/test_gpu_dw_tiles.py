@@ -1,4 +1,4 @@
-"""GPU: the cooperative weight-gradient schedule of gemm_tc.cu (MN_COOP).  One-plane MN-major split-K GEMMs with M >= 256
+"""GPU: the cooperative weight-gradient schedule of gemm_tc.cu (Sched::COOP).  One-plane MN-major split-K GEMMs with M >= 256
 run 256 x 128 items that both consumer warpgroups share and reduce into the fp32 output straight from the accumulator
 fragment; everything else keeps the 128 x 128 ping-pong items.  dW = dY^T X is compared against an fp64 product of the
 bf16-rounded operands, and the per-warpgroup item counters of the debug profile buffer show which schedule ran."""
