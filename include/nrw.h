@@ -71,6 +71,11 @@ NRW_API int nrw_ctx_set_backward_planes(nrw_ctx* ctx, int n);
 /* planes of the stored softplus outputs read by the BACKWARD sweeps to rebuild the gates softplus'(a), softplus''(a)
  * (0 = all forward planes; 1 halves that stream at ~1e-3 relative gate error).  The forward gradient chain always reads all. */
 NRW_API int nrw_ctx_set_backward_gate_planes(nrw_ctx* ctx, int n);
+/* on = 0: the background NeRF has no appearance head (models/nerf.py encode_appearance=False): its colour branch is
+ * relu(views_linears.0([feature, viewPE])) -> rgb_linear, the appearance code is neither read nor differentiated, and the
+ * nerf.apperence_encoding.* slots of the parameter table are unused (their gradient stays 0).  Default 1.  Call before
+ * nrw_ctx_bind: it changes the packed layout and the workspace (NRW_ERR_STATE after a bind). */
+NRW_API int nrw_ctx_set_nerf_appearance(nrw_ctx* ctx, int on);
 NRW_API long long nrw_packed_bytes(const nrw_ctx* ctx);
 /* n_slots_sdf / n_slots_nerf: how many chunks keep their forward activations resident for the backward pass
  * (>= number of chunks of a batch: no forward recompute in backward; 1: recompute, minimum memory). */

@@ -55,8 +55,18 @@ int nrw_ctx_create(nrw_ctx** out, int n_planes, int gemm_backend, int n_vocab, i
   NRW_CHECK(c != nullptr, NRW_ERR_ARG, "ctx_create: out of host memory");
   c->n_planes = n_planes; c->backend = gemm_backend; c->n_vocab = n_vocab; c->n_a = n_a;
   c->tab = build_param_table(n_vocab, n_a);
-  c->pm = build_packed_model(c->tab, n_planes);
+  c->pm = build_packed_model(c->tab, n_planes, true);
   *out = c;
+  return NRW_OK;
+  NRW_GUARD_END
+}
+int nrw_ctx_set_nerf_appearance(nrw_ctx* ctx, int on) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx && (on == 0 || on == 1), NRW_ERR_ARG, "set_nerf_appearance: on=%d must be 0 or 1", on);
+  NRW_CHECK(!ctx->bound, NRW_ERR_STATE,
+            "set_nerf_appearance: call before nrw_ctx_bind (it changes the packed layout and the workspace)");
+  ctx->nerf_app = on;
+  ctx->pm = build_packed_model(ctx->tab, ctx->n_planes, on != 0);
   return NRW_OK;
   NRW_GUARD_END
 }
@@ -159,7 +169,8 @@ int nrw_nerf_forward(nrw_ctx* ctx, const float* pts4, const float* dirs, const f
   c.use_nerf_slot(0);
   for (long long i = 0; i < n; i += c.Mc) {
     const int M = (int)((n - i) < c.Mc ? (n - i) : c.Mc);
-    NRW_TRY(nerf_chunk_forward(c, M, nullptr, dirs + i * 3, nullptr, nullptr, pts4 + i * 4, a + i * c.n_a, 1, 1, S(stream)));
+    NRW_TRY(nerf_chunk_forward(c, M, nullptr, dirs + i * 3, nullptr, nullptr, pts4 + i * 4,
+                               c.nerf_app ? a + i * c.n_a : nullptr, 1, 1, S(stream)));
     NRW_CUDA_OK(cudaMemcpyAsync(density + i, c.c_density, (size_t)M * 4, cudaMemcpyDeviceToDevice, S(stream)));
     NRW_CUDA_OK(cudaMemcpyAsync(rgb + i * 3, c.c_rgbbg, (size_t)M * 12, cudaMemcpyDeviceToDevice, S(stream)));
   }

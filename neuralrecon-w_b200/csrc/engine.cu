@@ -76,7 +76,7 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
       if (l != 5) s.NH[l] = fwd_planes(i, s0.NH[l], 256);
     s.IN5 = fwd_planes(i, s0.IN5, 384);
     s.FEATN = fwd_planes(i, s0.FEATN, 384);
-    for (int l = 1; l <= 4; ++l) s.AP[l] = fwd_planes(i, s0.AP[l], 128);
+    for (int l = 1; l <= (c.nerf_app ? 4 : 1); ++l) s.AP[l] = fwd_planes(i, s0.AP[l], 128);
     s.c_density = cv.f32(M);
     s.c_alpha = cv.f32(M);
     s.c_rgbbg = cv.f32(M * 3);
@@ -316,7 +316,8 @@ int nerf_chunk_forward(nrw_ctx& c, int M, const float* o, const float* d, const 
                        const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s) {
   c.cur_planes = c.n_planes;
   const int P = c.n_planes;
-  NRW_TRY(launch_nerf_embed(o, d, z, sdist, pts4, a, c.n_a, T, rows_per_src, M, P, c.IN0, c.IN5, c.FEATN,
+  // without the appearance head the code is not read: FEATN's a columns keep their zeros and meet zero weights
+  NRW_TRY(launch_nerf_embed(o, d, z, sdist, pts4, a, c.nerf_app ? c.n_a : 0, T, rows_per_src, M, P, c.IN0, c.IN5, c.FEATN,
                             pts4 ? nullptr : c.c_dists, s));
   { Epi e; e.bias = c.bias(L_N0); e.act = ACT_RELU; e.out_pl = c.NH[1]; NRW_TRY(mm(c, c.IN0, c.W(L_N0), M, 256, 128, e, s)); }
   for (int l = 1; l <= 3; ++l) {
@@ -332,12 +333,14 @@ int nerf_chunk_forward(nrw_ctx& c, int M, const float* o, const float* d, const 
   NRW_TRY(launch_head(1, c.NH[8], P, 256, M, c.f_area + c.pm.heads.na_w, c.f_area + c.pm.heads.na_b, ACT_NONE,
                       pts4 ? nullptr : c.c_dists, pts4 ? c.c_density : c.c_alpha, pts4 ? nullptr : c.c_density, s));
   { Epi e; e.bias = c.bias(L_NF); e.out_pl = c.FEATN; NRW_TRY(mm(c, c.NH[8], c.W(L_NF), M, 256, 256, e, s)); }
+  // L_NS0 is static_linear_0 of the appearance head, or views_linears.0 without it (the last layer before rgb_linear)
   { Epi e; e.bias = c.bias(L_NS0); e.act = ACT_RELU; e.out_pl = c.AP[1]; NRW_TRY(mm(c, c.FEATN, c.W(L_NS0), M, 128, 384, e, s)); }
-  for (int l = 1; l <= 3; ++l) {
+  const int last = c.nerf_app ? 4 : 1;
+  for (int l = 1; l < last; ++l) {
     Epi e; e.bias = c.bias(L_NS0 + l); e.act = ACT_RELU; e.out_pl = c.AP[l + 1];
     NRW_TRY(mm(c, c.AP[l], c.W(L_NS0 + l), M, 128, 128, e, s));
   }
-  NRW_TRY(launch_head(3, c.AP[4], P, 128, M, c.f_area + c.pm.heads.nr_w, c.f_area + c.pm.heads.nr_b, ACT_NONE, nullptr,
+  NRW_TRY(launch_head(3, c.AP[last], P, 128, M, c.f_area + c.pm.heads.nr_w, c.f_area + c.pm.heads.nr_b, ACT_NONE, nullptr,
                       c.c_rgbbg, nullptr, s));
   return NRW_OK;
 }
@@ -448,20 +451,23 @@ int nerf_chunk_backward(nrw_ctx& c, int M, const float* d_bga, const float* d_bg
   c.cur_planes = c.bwd_planes > 0 ? c.bwd_planes : c.n_planes;   // 'mixed' mode: backward GEMMs in plain bf16
   const int P = c.cur_planes;
   const Heads& H = c.pm.heads;
-  NRW_TRY(launch_head_bwd(3, c.AP[4], P, 128, M, c.f_area + H.nr_w, d_bgc, nullptr, nullptr, 0, c.dNA[0], nullptr,
+  const int last = c.nerf_app ? 4 : 1;   // layers L_NS0 .. L_NS0 + last - 1 feed rgb_linear (nerf_chunk_forward)
+  NRW_TRY(launch_head_bwd(3, c.AP[last], P, 128, M, c.f_area + H.nr_w, d_bgc, nullptr, nullptr, 0, c.dNA[0], nullptr,
                           c.gs + H.d_nr_w, c.gs + H.d_nr_b, s));
   int cur = 0;
-  NRW_TRY(bias_grad(c, c.dNA[0], M, L_NS0 + 3, s));
-  for (int l = 3; l >= 1; --l) {
+  NRW_TRY(bias_grad(c, c.dNA[0], M, L_NS0 + last - 1, s));
+  for (int l = last - 1; l >= 1; --l) {
     Epi e; e.aux_relu = c.AP[l].p; e.ld_relu = 128; e.out_pl = c.dNA[1 - cur]; e.colsum = c.db(L_NS0 + l - 1);
     NRW_TRY(mm_bwd(c, c.dNA[cur], c.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
     cur = 1 - cur;
   }
   { Epi e; e.out_pl = c.dNF; e.colsum = c.db(L_NF);
     NRW_TRY(mm_bwd(c, c.dNA[cur], c.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
-  { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
-    NRW_TRY(mm(c, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
-  if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, T, d_a_rays, 1, s));
+  if (c.nerf_app) {   // the appearance code's gradient: FEATN columns 283.. of L_NS0
+    { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
+      NRW_TRY(mm(c, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
+    if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, T, d_a_rays, 1, s));
+  }
   // alpha head -> d_density
   NRW_TRY(launch_head_bwd(1, c.NH[8], P, 256, M, c.f_area + H.na_w, d_bga, c.c_density, c.c_dists, 2,
                           Planes{nullptr, 0, 0}, c.c_ddens, c.gs + H.d_na_w, c.gs + H.d_na_b, s));

@@ -28,6 +28,7 @@ struct nrw_ctx {
   int cur_planes = 2;   // planes used by the GEMM helpers of the pass in flight
   int bwd_gate_planes = 0;   // planes of u read for the softplus gates of the BACKWARD sweeps (0 = all forward planes)
   int gate_planes() const { return bwd_gate_planes > 0 ? bwd_gate_planes : n_planes; }
+  int nerf_app = 1;     // 0: background NeRF without appearance head (nrw_ctx_set_nerf_appearance)
   std::vector<FwdSdfSlot> sdf_slots;
   std::vector<FwdNerfSlot> nerf_slots;
   int n_slots_sdf = 1, n_slots_nerf = 1;

@@ -95,7 +95,7 @@ static void finish_layer(PackedLayer& L) {
     if (L.colmap[j] >= 0) L.colinv[L.colmap[j]] = (short)j;
 }
 
-PackedModel build_packed_model(const std::vector<ParamInfo>& tab, int n_planes) {
+PackedModel build_packed_model(const std::vector<ParamInfo>& tab, int n_planes, bool nerf_app) {
   PackedModel pm;
   memset(&pm, 0, sizeof(pm));
   PackedLayer* L = pm.layers;
@@ -128,9 +128,12 @@ PackedModel build_packed_model(const std::vector<ParamInfo>& tab, int n_planes) 
     for (int j = 0; j < 84; ++j) c.colmap[256 + j] = (short)j;
   }
   init_layer(L[L_NF], tab, PI_NF_W, -1, PI_NF_B, 0, 256, 256, 256);
-  init_layer(L[L_NS0], tab, PI_NAPP_BASE, -1, PI_NAPP_BASE + 1, 0, 128, 128, 384);  // [feat256|viewPE27|a|pad]
-  for (int s = 1; s < 4; ++s)
-    init_layer(L[L_NS0 + s], tab, PI_NAPP_BASE + 2 * s, -1, PI_NAPP_BASE + 2 * s + 1, 0, 128, 128, 128);
+  if (nerf_app)
+    init_layer(L[L_NS0], tab, PI_NAPP_BASE, -1, PI_NAPP_BASE + 1, 0, 128, 128, 384);  // [feat256|viewPE27|a|pad]
+  else   // views_linears.0 over [feat256|viewPE27]: the a and pad columns of FEATN meet zero weights
+    init_layer(L[L_NS0], tab, PI_NVIEWS_W, -1, PI_NVIEWS_B, 0, 128, 128, 384);
+  for (int s = 1; s < 4; ++s)   // (no rows without appearance: packed as zeros, no gradient unpacked)
+    init_layer(L[L_NS0 + s], tab, PI_NAPP_BASE + 2 * s, -1, PI_NAPP_BASE + 2 * s + 1, 0, nerf_app ? 128 : 0, 128, 128);
   for (int i = 0; i < L_COUNT; ++i) finish_layer(L[i]);
 
   // packed buffer layout: [device copy of layer table][bf16 area][fp32 area]

@@ -86,7 +86,9 @@ struct PackedModel {
   long long plane_stride[L_COUNT];   // bf16 elements between planes of W (== Np*Kp), same for WT
   long long grad_floats;      // size of the gradient scratch (dWp/dbp/head grads), floats
 };
-PackedModel build_packed_model(const std::vector<ParamInfo>& tab, int n_planes);
+// nerf_app = 0: the background NeRF without appearance codes (nerf.py encode_appearance=False) - L_NS0 packs
+// views_linears.0 and L_NS1..L_NS3 hold no rows (same sizes, so the packed layout does not depend on the flag)
+PackedModel build_packed_model(const std::vector<ParamInfo>& tab, int n_planes, bool nerf_app);
 
 int pack_weights(const PackedModel& pm, const std::vector<ParamInfo>& tab, int n_planes, const float* params,
                  void* packed_base, cudaStream_t s);

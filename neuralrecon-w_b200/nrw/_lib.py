@@ -83,6 +83,7 @@ def lib():
     L.nrw_ctx_destroy.argtypes = [vp]
     L.nrw_ctx_set_backward_planes.argtypes = [vp, i32]
     L.nrw_ctx_set_backward_gate_planes.argtypes = [vp, i32]
+    L.nrw_ctx_set_nerf_appearance.argtypes = [vp, i32]
     L.nrw_packed_bytes.restype = ll
     L.nrw_packed_bytes.argtypes = [vp]
     L.nrw_workspace_bytes.restype = ll
@@ -178,7 +179,7 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_reproject_mark", "nrw_raygen_capacity", "nrw_raygen_scratch_bytes", "nrw_raygen_image",
            "nrw_depth_range_scratch_bytes", "nrw_depth_range", "nrw_voxel_cast", "nrw_voxel_lookup",
            "nrw_view_roi_count", "nrw_label_static_count", "nrw_first_hit_scratch_bytes", "nrw_first_hit",
-           "nrw_obs_reproj_error"]
+           "nrw_obs_reproj_error", "nrw_ctx_set_nerf_appearance"]
 
 
 def check(status, what=""):

@@ -44,6 +44,8 @@ class Engine:
         self.ctx = C.c_void_p()
         check(self.L.nrw_ctx_create(C.byref(self.ctx), self.n_planes, self.backend, self.n_vocab, self.n_a),
               "nrw_ctx_create")
+        if nerf is not None and not nerf.encode_appearance:
+            check(self.L.nrw_ctx_set_nerf_appearance(self.ctx, 0), "nrw_ctx_set_nerf_appearance")
         if self.bwd_planes:
             check(self.L.nrw_ctx_set_backward_planes(self.ctx, self.bwd_planes), "nrw_ctx_set_backward_planes")
         # backward sweeps rebuild softplus'(a) / softplus''(a) from the stored output planes: with plain-bf16 backward GEMMs
@@ -208,9 +210,10 @@ class Engine:
         self.pack(dev)
         dens = torch.empty(n, 1, dtype=torch.float32, device=dev)
         rgb = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        # without the appearance head the code is not read (it may be None)
+        a_c = a.detach().reshape(n, -1).contiguous().float() if self.nerf.encode_appearance else None
         check(self.L.nrw_nerf_forward(self.ctx, ptr(pts4), ptr(dirs.detach().reshape(-1, 3).contiguous().float()),
-                                      ptr(a.detach().reshape(n, -1).contiguous().float()), n, ptr(dens), ptr(rgb),
-                                      stream_ptr()), "nrw_nerf_forward")
+                                      ptr(a_c), n, ptr(dens), ptr(rgb), stream_ptr()), "nrw_nerf_forward")
         return dens, rgb
 
     def sample(self, scfg, o, d, near, far, s_near=None, s_far=None, u_ray=None, u_out=None, trace=False):

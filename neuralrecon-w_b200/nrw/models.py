@@ -155,26 +155,31 @@ class NeuconW(nn.Module):
 
 
 class NeRF(nn.Module):
-    """Background field, models/nerf.py:86-184 (D=8, W=256, 4-D inverted-sphere input, appearance head)."""
+    """Background field, models/nerf.py:86-184 (D=8, W=256, 4-D inverted-sphere input).  With encode_appearance the
+    colour branch is the 4-layer appearance head over [feature, viewPE, a]; without it (config/train_indoor.yaml,
+    ENCODE_A_BG: False) it is relu(views_linears.0([feature, viewPE])), there is no apperence_encoding and the
+    appearance code passed to forward is ignored."""
 
     def __init__(self, D=8, W=256, d_in=3, d_in_view=3, multires=0, multires_view=0, output_ch=4, skips=[4],
                  in_channels_a=48, in_channels_dir=27, encode_appearance=False, use_viewdirs=False):
         super().__init__()
-        if (D, W, d_in, d_in_view, multires, multires_view, list(skips), in_channels_dir, bool(encode_appearance),
-                bool(use_viewdirs)) != (8, 256, 4, 3, 10, 4, [4], 27, True, True):
+        if (D, W, d_in, d_in_view, multires, multires_view, list(skips), in_channels_dir,
+                bool(use_viewdirs)) != (8, 256, 4, 3, 10, 4, [4], 27, True):
             raise NrwError("NeRF: the CUDA path implements D=8, W=256, d_in=4, multires=10, multires_view=4, "
-                           "skips=[4], encode_appearance=True, use_viewdirs=True only")
+                           "skips=[4], use_viewdirs=True only")
         self.D, self.W, self.in_channels_a, self.in_channels_dir = D, W, in_channels_a, in_channels_dir
         self.input_ch, self.input_ch_view = 84, 27
-        self.skips, self.use_viewdirs, self.encode_appearance = skips, use_viewdirs, encode_appearance
+        self.skips, self.use_viewdirs, self.encode_appearance = skips, use_viewdirs, bool(encode_appearance)
         self.pts_linears = nn.ModuleList(
             [nn.Linear(self.input_ch, W)] +
             [nn.Linear(W, W) if i not in skips else nn.Linear(W + self.input_ch, W) for i in range(D - 1)])
-        enc = OrderedDict([("static_linear_0", nn.Linear(W + in_channels_dir + in_channels_a, W // 2))])
-        for s in range(1, D // 2):
-            enc[f"static_linear_{s}"] = nn.Linear(W // 2, W // 2)
-        self.apperence_encoding = nn.Sequential(enc)
-        self.views_linears = nn.ModuleList([nn.Linear(self.input_ch_view + W, W // 2)])  # unused, kept (nerf.py:143)
+        if self.encode_appearance:
+            enc = OrderedDict([("static_linear_0", nn.Linear(W + in_channels_dir + in_channels_a, W // 2))])
+            for s in range(1, D // 2):
+                enc[f"static_linear_{s}"] = nn.Linear(W // 2, W // 2)
+            self.apperence_encoding = nn.Sequential(enc)
+        # live only without the appearance head; kept either way, as the reference does (nerf.py:143)
+        self.views_linears = nn.ModuleList([nn.Linear(self.input_ch_view + W, W // 2)])
         self.feature_linear = nn.Linear(W, W)
         self.alpha_linear = nn.Linear(W, 1)
         self.rgb_linear = nn.Linear(W // 2, 3)

@@ -89,13 +89,18 @@ class TrainSystem:
     def __init__(self, device, n_samples=64, n_importance=64, up_sample_steps=4, n_outside=4, s_val_base=3,
                  n_vocab=5000, n_a=48, origin=(0.0, 0.0, 0.0), radius=1.0, precision=None, chunk_rows=None,
                  batch_size=8192, world_size=1, canonical_lr=1e-4, canonical_bs=4096, anneal_end=50000,
-                 igr_weight=0.0001, mask_weight=0.1, depth_weight=0.1, seed=66, fused_optimizer=True):
+                 igr_weight=0.0001, mask_weight=0.1, depth_weight=0.1, seed=66, fused_optimizer=True, encode_a_bg=True,
+                 inside_outside=False):
+        """encode_a_bg / inside_outside: NEUCONW.ENCODE_A_BG and SDF_CONFIG.inside_outside (config/train_indoor.yaml sets
+        False / True: a background NeRF without appearance codes, and the SDF's geometric init flipped for a scene seen
+        from inside)."""
         torch.manual_seed(seed)
         self.device = device
         self.embedding_a = torch.nn.Embedding(n_vocab, n_a).to(device)
-        self.neuconw = NeuconW(SDF_CONFIG, COLOR_CONFIG, dict(init_val=0.3), in_channels_a=n_a, encode_a=True).to(device)
+        self.neuconw = NeuconW(dict(SDF_CONFIG, inside_outside=bool(inside_outside)), COLOR_CONFIG, dict(init_val=0.3),
+                               in_channels_a=n_a, encode_a=True).to(device)
         self.nerf = NeRF(D=8, d_in=4, d_in_view=3, W=256, multires=10, multires_view=4, output_ch=4, skips=[4],
-                         encode_appearance=True, in_channels_a=n_a, in_channels_dir=27, use_viewdirs=True).to(device)
+                         encode_appearance=bool(encode_a_bg), in_channels_a=n_a, in_channels_dir=27, use_viewdirs=True).to(device)
         self.renderer = NeuconWRenderer(
             nerf=self.nerf, neuconw=self.neuconw, embeddings={"a": self.embedding_a}, n_samples=n_samples,
             s_val_base=s_val_base, n_importance=n_importance, n_outside=n_outside, up_sample_steps=up_sample_steps,
