@@ -18,7 +18,6 @@ using namespace nrw;
   }
 
 static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s); }
-static long long g_aux_launches = 0;
 
 extern "C" {
 
@@ -54,6 +53,7 @@ int nrw_ctx_create(nrw_ctx** out, int n_planes, int gemm_backend, int n_vocab, i
   nrw_ctx* c = new (std::nothrow) nrw_ctx();
   NRW_CHECK(c != nullptr, NRW_ERR_ARG, "ctx_create: out of host memory");
   c->n_planes = n_planes; c->backend = gemm_backend; c->n_vocab = n_vocab; c->n_a = n_a;
+  c->bwd_planes = c->bwd_gate_planes = n_planes;
   c->tab = build_param_table(n_vocab, n_a);
   c->pm = build_packed_model(c->tab, n_planes, true);
   *out = c;
@@ -74,11 +74,11 @@ int nrw_ctx_set_backward_planes(nrw_ctx* ctx, int n) {
   NRW_GUARD_BEGIN
   NRW_CHECK(ctx && n >= 0 && n <= ctx->n_planes, NRW_ERR_ARG, "set_backward_planes: n=%d out of range", n);
   NRW_CHECK(!ctx->bound, NRW_ERR_STATE, "set_backward_planes: call before nrw_ctx_bind (it changes the workspace layout)");
-  ctx->bwd_planes = n;
+  ctx->bwd_planes = n ? n : ctx->n_planes;
   // plain-bf16 backward: the fp32 side streams only the backward pass reads (Q_l of the gradient chain, the second-order
   // terms of the tangent sweep) are kept as ONE bf16 plane as well - their consumers multiply them into bf16 operands
   const char* env = getenv("NRW_AUX_BF16");
-  ctx->aux_bf16 = n == 1 && ctx->n_planes > 1 && ctx->backend == NRW_GEMM_TCGEN05 && !(env && atoi(env) == 0);
+  ctx->aux_bf16 = ctx->bwd_planes == 1 && ctx->n_planes > 1 && ctx->backend == NRW_GEMM_TCGEN05 && !(env && atoi(env) == 0);
   return NRW_OK;
   NRW_GUARD_END
 }
@@ -86,7 +86,7 @@ int nrw_ctx_set_backward_gate_planes(nrw_ctx* ctx, int n) {
   NRW_GUARD_BEGIN
   NRW_CHECK(ctx != nullptr && n >= 0 && n <= ctx->n_planes, NRW_ERR_ARG, "set_backward_gate_planes: n=%d outside 0..n_planes", n);
   NRW_CHECK(!ctx->bound, NRW_ERR_STATE, "set_backward_gate_planes: call before nrw_ctx_bind (it changes the workspace layout)");
-  ctx->bwd_gate_planes = n;
+  ctx->bwd_gate_planes = n ? n : ctx->n_planes;
   return NRW_OK;
   NRW_GUARD_END
 }
@@ -124,7 +124,6 @@ int nrw_pack_weights(nrw_ctx* ctx, const float* params, void* stream) {
   NRW_TRY(pack_weights(ctx->pm, ctx->tab, ctx->n_planes, params, ctx->packed, S(stream)));
   ctx->params = params;
   ctx->packed_valid = true;
-  g_aux_launches += 2;
   return NRW_OK;
   NRW_GUARD_END
 }
@@ -141,21 +140,7 @@ int nrw_neuconw_forward(nrw_ctx* ctx, const float* pts, const float* dirs, const
                         float* sdf, float* normals, void* stream) {
   NRW_GUARD_BEGIN
   NRW_CHECK(ctx && ctx->bound && ctx->packed_valid, NRW_ERR_STATE, "neuconw_forward: bind + pack first");
-  nrw_ctx& c = *ctx;
-  c.fwd_cached = false;  // slot 0 is reused
-  c.use_sdf_slot(0);
-  c.use_nerf_slot(0);
-  for (long long i = 0; i < n; i += c.Mc) {
-    const int M = (int)((n - i) < c.Mc ? (n - i) : c.Mc);
-    NRW_TRY(sdf_chunk_forward(c, M, pts + i * 3, true, rgb != nullptr, S(stream)));
-    if (rgb) {
-      NRW_TRY(color_chunk_forward(c, M, pts + i * 3, dirs + i * 3, a + i * c.n_a, 1, S(stream)));
-      NRW_CUDA_OK(cudaMemcpyAsync(rgb + i * 3, c.c_rgb, (size_t)M * 12, cudaMemcpyDeviceToDevice, S(stream)));
-    }
-    if (sdf) NRW_CUDA_OK(cudaMemcpyAsync(sdf + i, c.c_sdf, (size_t)M * 4, cudaMemcpyDeviceToDevice, S(stream)));
-    if (normals) NRW_CUDA_OK(cudaMemcpyAsync(normals + i * 3, c.c_nrm, (size_t)M * 12, cudaMemcpyDeviceToDevice, S(stream)));
-  }
-  return NRW_OK;
+  return neuconw_query(*ctx, pts, dirs, a, n, rgb, sdf, normals, S(stream));
   NRW_GUARD_END
 }
 
@@ -163,18 +148,7 @@ int nrw_nerf_forward(nrw_ctx* ctx, const float* pts4, const float* dirs, const f
                      float* rgb, void* stream) {
   NRW_GUARD_BEGIN
   NRW_CHECK(ctx && ctx->bound && ctx->packed_valid, NRW_ERR_STATE, "nerf_forward: bind + pack first");
-  nrw_ctx& c = *ctx;
-  c.fwd_cached = false;  // slot 0 is reused
-  c.use_sdf_slot(0);
-  c.use_nerf_slot(0);
-  for (long long i = 0; i < n; i += c.Mc) {
-    const int M = (int)((n - i) < c.Mc ? (n - i) : c.Mc);
-    NRW_TRY(nerf_chunk_forward(c, M, nullptr, dirs + i * 3, nullptr, nullptr, pts4 + i * 4,
-                               c.nerf_app ? a + i * c.n_a : nullptr, 1, 1, S(stream)));
-    NRW_CUDA_OK(cudaMemcpyAsync(density + i, c.c_density, (size_t)M * 4, cudaMemcpyDeviceToDevice, S(stream)));
-    NRW_CUDA_OK(cudaMemcpyAsync(rgb + i * 3, c.c_rgbbg, (size_t)M * 12, cudaMemcpyDeviceToDevice, S(stream)));
-  }
-  return NRW_OK;
+  return nerf_query(*ctx, pts4, dirs, a, n, density, rgb, S(stream));
   NRW_GUARD_END
 }
 

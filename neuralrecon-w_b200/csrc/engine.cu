@@ -2,7 +2,8 @@
 // colour net -> compositing, and the hand-derived backward of all of it (SURVEY.md 9.2/9.3).
 // Every dense layer is one tensor-core GEMM launch with a fused epilogue; chunks of `Mc` samples keep the
 // inter-layer activations L2-resident.  Backward consumes a chunk's forward from its slot; chunks that found no slot of
-// their own are recomputed into the workspace and consumed at once, so memory is O(slots x chunk), not O(batch).
+// their own are recomputed into the last slot and consumed at once (chunk_visit), so memory is O(slots x chunk), not
+// O(batch).
 #include <stdlib.h>
 
 #include "engine.h"
@@ -39,7 +40,7 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
   // In 'mixed' nothing after a chunk's own forward reads the lo plane of its activations: the backward GEMMs, gates, ReLU
   // masks and heads all run on the hi plane.  So slots 1.. keep only the hi plane of each two-plane tensor and point their
   // plane 1 (pstride = lo - hi, negative) at slot 0's lo plane, which every slot shares as scratch.
-  const bool shared_lo = P == 2 && c.bwd_planes == 1 && c.gate_planes() == 1;
+  const bool shared_lo = P == 2 && c.bwd_planes == 1 && c.bwd_gate_planes == 1;
   auto fwd_planes = [&](int slot, const Planes& slot0, int ld) {
     if (slot == 0 || !shared_lo) return cv.planes(M, ld, P);
     Planes h = cv.planes(M, ld, 1);
@@ -82,14 +83,10 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
     s.c_rgbbg = cv.f32(M * 3);
     s.c_dists = cv.f32(M);
   }
-  c.n_slots_sdf = n_slots_sdf;
-  c.n_slots_nerf = n_slots_nerf;
-  c.use_sdf_slot(0);
-  c.use_nerf_slot(0);
   c.fwd_cached = false;
   c.ge_acc = cv.f32(4);
   if (with_bwd) {
-    const int PB = c.bwd_planes > 0 ? c.bwd_planes : P;   // the backward writes and reads only its own planes
+    const int PB = c.bwd_planes;   // the backward writes and reads only its own planes
     c.DQ0 = cv.planes(M, 64, PB);
     c.DQodd = cv.planes(M, 512, PB);
     c.DQeven = cv.planes(M, 512, PB);
@@ -220,8 +217,8 @@ static int bias_grad(nrw_ctx& c, Planes dY, int M, int layer, cudaStream_t s) {
 }
 // gate of SDF layer l (softplus'(a_l), softplus''(a_l)) from the planes of u_{l+1} = softplus(a_l): U[l+1] holds
 // softplus(a_l) (x 1/sqrt2 in its first 473 columns for l == 3, the skip layer's input)
-static void gate_from(nrw_ctx& c, Epi& e, int l, int planes) {
-  e.aux_u = c.U[l + 1];
+static void gate_from(const FwdSdfSlot& f, Epi& e, int l, int planes) {
+  e.aux_u = f.U[l + 1];
   e.aux_u_planes = planes;
   e.aux_u_scale = (l == 3) ? 1.41421356237309504880f : 1.0f;
 }
@@ -246,10 +243,11 @@ static int sdf_fused_query(nrw_ctx& c, const float* pts, int M, float* sdf, cuda
   return sdf_fused_forward(d, s);
 }
 
-int sdf_chunk_forward(nrw_ctx& c, int M, const float* pts, bool need_normal, bool need_feat, cudaStream_t s) {
+int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool need_normal, bool need_feat,
+                      cudaStream_t s) {
   c.cur_planes = c.n_planes;
   const int P = c.n_planes;
-  NRW_TRY(launch_sdf_embed(pts, M, P, c.U0, c.U[4], s));
+  NRW_TRY(launch_sdf_embed(pts, M, P, f.U0, f.U[4], s));
   const float* w0 = c.f_area + c.pm.heads.sdf_w0;
   const float* b0 = c.f_area + c.pm.heads.sdf_b0;
   // forward-only query (sampler, NeuconWRenderer.sdf, mesh / refresh pipelines): the SDF head is fused into the epilogue of
@@ -257,91 +255,91 @@ int sdf_chunk_forward(nrw_ctx& c, int M, const float* pts, bool need_normal, boo
   const bool fused_head = !need_normal && !need_feat && M >= 256 && c.backend == NRW_GEMM_TCGEN05;
   // NRW_SDF_FUSED=1: the whole forward-only chain (encoding, 8 layers, head) as ONE kernel with the activations resident in
   // shared memory (gemm_tc.cu::sdf_fused_kernel) - two-plane operands only
-  if (fused_head && sdf_fused_enabled(c)) return sdf_fused_query(c, pts, M, c.c_sdf, s);
+  if (fused_head && sdf_fused_enabled(c)) return sdf_fused_query(c, pts, M, f.c_sdf, s);
   for (int l = 0; l < 8; ++l) {
     Epi e;
     e.bias = c.bias(L_SDF0 + l);
     e.act = ACT_SOFTPLUS100;
     // (no fp32 pre-activation store: every later gate softplus'(a_l), softplus''(a_l) is recomputed from the planes of
     //  u_{l+1} = softplus(a_l) that the next layer needs anyway - common.cuh softplus100_d12_from_u)
-    if (l == 7 && fused_head) { e.head_w = w0; e.head_partial = c.HP; }
-    else e.out_pl = c.U[l + 1];
+    if (l == 7 && fused_head) { e.head_w = w0; e.head_partial = f.HP; }
+    else e.out_pl = f.U[l + 1];
     if (l == 3) { e.scale = INV_SQRT2; e.n_store = 473; }
-    NRW_TRY(mm(c, l == 0 ? c.U0 : c.U[l], c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
+    NRW_TRY(mm(c, l == 0 ? f.U0 : f.U[l], c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
   }
-  if (fused_head) NRW_TRY(launch_sdf_head_sum(c.HP, M, b0, c.c_sdf, s));
-  else NRW_TRY(launch_sdf_head(c.U[8], M, w0, b0, c.c_sdf, P, need_normal ? c.G[7] : Planes{nullptr, 0, 0}, s));
+  if (fused_head) NRW_TRY(launch_sdf_head_sum(f.HP, M, b0, f.c_sdf, s));
+  else NRW_TRY(launch_sdf_head(f.U[8], M, w0, b0, f.c_sdf, P, need_normal ? f.G[7] : Planes{nullptr, 0, 0}, s));
   if (need_feat) {
     Epi e;
     e.bias = c.bias(L_SDF8F);
-    e.out_pl = c.FEAT;
-    NRW_TRY(mm(c, c.U[8], c.W(L_SDF8F), M, 512, 512, e, s));
+    e.out_pl = f.FEAT;
+    NRW_TRY(mm(c, f.U[8], c.W(L_SDF8F), M, 512, 512, e, s));
   }
   if (need_normal) {
     for (int l = 7; l >= 1; --l) {
       Epi e;
-      e.out_pre = c.Q[l];
-      gate_from(c, e, l - 1, c.n_planes);
-      e.out_pl = c.G[l - 1];
+      e.out_pre = f.Q[l];
+      gate_from(f, e, l - 1, c.n_planes);
+      e.out_pl = f.G[l - 1];
       if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }
-      NRW_TRY(mm(c, c.G[l], c.WT(L_SDF0 + l), M, 512, 512, e, s));
+      NRW_TRY(mm(c, f.G[l], c.WT(L_SDF0 + l), M, 512, 512, e, s));
     }
     Epi e;
-    e.out_pre = c.Q[0];
-    NRW_TRY(mm(c, c.G[0], c.WT(L_SDF0), M, 64, 512, e, s));
-    NRW_TRY(launch_sdf_normal(pts, c.Q[0].f32(), c.Q[4].f32(), M, c.c_nrm, s));
+    e.out_pre = f.Q[0];
+    NRW_TRY(mm(c, f.G[0], c.WT(L_SDF0), M, 64, 512, e, s));
+    NRW_TRY(launch_sdf_normal(pts, f.Q[0].f32(), f.Q[4].f32(), M, f.c_nrm, s));
   }
   return NRW_OK;
 }
 
-int color_chunk_forward(nrw_ctx& c, int M, const float* pts, const float* dirs, const float* a, int rows_per_src,
-                        cudaStream_t s) {
+int color_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, const float* dirs, const float* a,
+                        int rows_per_src, cudaStream_t s) {
   c.cur_planes = c.n_planes;
   const int P = c.n_planes;
-  NRW_TRY(launch_color_embed(dirs, a, c.n_a, rows_per_src, pts, c.c_nrm, M, P, c.IN1, c.IN2, s));
-  { Epi e; e.bias = c.bias(L_CX); e.out_pl = c.IN1; NRW_TRY(mm(c, c.FEAT, c.W(L_CX), M, 512, 512, e, s)); }
-  { Epi e; e.bias = c.bias(L_CS0); e.act = ACT_RELU; e.out_pl = c.H1; NRW_TRY(mm(c, c.IN1, c.W(L_CS0), M, 128, 640, e, s)); }
-  { Epi e; e.bias = c.bias(L_CS1); e.act = ACT_RELU; e.out_pl = c.IN2; NRW_TRY(mm(c, c.H1, c.W(L_CS1), M, 128, 128, e, s)); }
-  { Epi e; e.bias = c.bias(L_CL0); e.act = ACT_RELU; e.out_pl = c.X[1]; NRW_TRY(mm(c, c.IN2, c.W(L_CL0), M, 256, 192, e, s)); }
+  NRW_TRY(launch_color_embed(dirs, a, c.n_a, rows_per_src, pts, f.c_nrm, M, P, f.IN1, f.IN2, s));
+  { Epi e; e.bias = c.bias(L_CX); e.out_pl = f.IN1; NRW_TRY(mm(c, f.FEAT, c.W(L_CX), M, 512, 512, e, s)); }
+  { Epi e; e.bias = c.bias(L_CS0); e.act = ACT_RELU; e.out_pl = f.H1; NRW_TRY(mm(c, f.IN1, c.W(L_CS0), M, 128, 640, e, s)); }
+  { Epi e; e.bias = c.bias(L_CS1); e.act = ACT_RELU; e.out_pl = f.IN2; NRW_TRY(mm(c, f.H1, c.W(L_CS1), M, 128, 128, e, s)); }
+  { Epi e; e.bias = c.bias(L_CL0); e.act = ACT_RELU; e.out_pl = f.X[1]; NRW_TRY(mm(c, f.IN2, c.W(L_CL0), M, 256, 192, e, s)); }
   for (int l = 1; l <= 3; ++l) {
-    Epi e; e.bias = c.bias(L_CL0 + l); e.act = ACT_RELU; e.out_pl = c.X[l + 1];
-    NRW_TRY(mm(c, c.X[l], c.W(L_CL0 + l), M, 256, 256, e, s));
+    Epi e; e.bias = c.bias(L_CL0 + l); e.act = ACT_RELU; e.out_pl = f.X[l + 1];
+    NRW_TRY(mm(c, f.X[l], c.W(L_CL0 + l), M, 256, 256, e, s));
   }
-  NRW_TRY(launch_head(3, c.X[4], P, 256, M, c.f_area + c.pm.heads.cl4_w, c.f_area + c.pm.heads.cl4_b, ACT_SIGMOID,
-                      nullptr, c.c_rgb, nullptr, s));
+  NRW_TRY(launch_head(3, f.X[4], P, 256, M, c.f_area + c.pm.heads.cl4_w, c.f_area + c.pm.heads.cl4_b, ACT_SIGMOID,
+                      nullptr, f.c_rgb, nullptr, s));
   return NRW_OK;
 }
 
-int nerf_chunk_forward(nrw_ctx& c, int M, const float* o, const float* d, const float* z, const float* sdist,
-                       const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s) {
+int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const float* d, const float* z,
+                       const float* sdist, const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s) {
   c.cur_planes = c.n_planes;
   const int P = c.n_planes;
   // without the appearance head the code is not read: FEATN's a columns keep their zeros and meet zero weights
-  NRW_TRY(launch_nerf_embed(o, d, z, sdist, pts4, a, c.nerf_app ? c.n_a : 0, T, rows_per_src, M, P, c.IN0, c.IN5, c.FEATN,
-                            pts4 ? nullptr : c.c_dists, s));
-  { Epi e; e.bias = c.bias(L_N0); e.act = ACT_RELU; e.out_pl = c.NH[1]; NRW_TRY(mm(c, c.IN0, c.W(L_N0), M, 256, 128, e, s)); }
+  NRW_TRY(launch_nerf_embed(o, d, z, sdist, pts4, a, c.nerf_app ? c.n_a : 0, T, rows_per_src, M, P, f.IN0, f.IN5, f.FEATN,
+                            pts4 ? nullptr : f.c_dists, s));
+  { Epi e; e.bias = c.bias(L_N0); e.act = ACT_RELU; e.out_pl = f.NH[1]; NRW_TRY(mm(c, f.IN0, c.W(L_N0), M, 256, 128, e, s)); }
   for (int l = 1; l <= 3; ++l) {
-    Epi e; e.bias = c.bias(L_N0 + l); e.act = ACT_RELU; e.out_pl = c.NH[l + 1];
-    NRW_TRY(mm(c, c.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
+    Epi e; e.bias = c.bias(L_N0 + l); e.act = ACT_RELU; e.out_pl = f.NH[l + 1];
+    NRW_TRY(mm(c, f.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
   }
-  { Epi e; e.bias = c.bias(L_N0 + 4); e.act = ACT_RELU; e.out_pl = c.IN5; NRW_TRY(mm(c, c.NH[4], c.W(L_N0 + 4), M, 256, 256, e, s)); }
-  { Epi e; e.bias = c.bias(L_N0 + 5); e.act = ACT_RELU; e.out_pl = c.NH[6]; NRW_TRY(mm(c, c.IN5, c.W(L_N0 + 5), M, 256, 384, e, s)); }
+  { Epi e; e.bias = c.bias(L_N0 + 4); e.act = ACT_RELU; e.out_pl = f.IN5; NRW_TRY(mm(c, f.NH[4], c.W(L_N0 + 4), M, 256, 256, e, s)); }
+  { Epi e; e.bias = c.bias(L_N0 + 5); e.act = ACT_RELU; e.out_pl = f.NH[6]; NRW_TRY(mm(c, f.IN5, c.W(L_N0 + 5), M, 256, 384, e, s)); }
   for (int l = 6; l <= 7; ++l) {
-    Epi e; e.bias = c.bias(L_N0 + l); e.act = ACT_RELU; e.out_pl = c.NH[l + 1];
-    NRW_TRY(mm(c, c.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
+    Epi e; e.bias = c.bias(L_N0 + l); e.act = ACT_RELU; e.out_pl = f.NH[l + 1];
+    NRW_TRY(mm(c, f.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
   }
-  NRW_TRY(launch_head(1, c.NH[8], P, 256, M, c.f_area + c.pm.heads.na_w, c.f_area + c.pm.heads.na_b, ACT_NONE,
-                      pts4 ? nullptr : c.c_dists, pts4 ? c.c_density : c.c_alpha, pts4 ? nullptr : c.c_density, s));
-  { Epi e; e.bias = c.bias(L_NF); e.out_pl = c.FEATN; NRW_TRY(mm(c, c.NH[8], c.W(L_NF), M, 256, 256, e, s)); }
+  NRW_TRY(launch_head(1, f.NH[8], P, 256, M, c.f_area + c.pm.heads.na_w, c.f_area + c.pm.heads.na_b, ACT_NONE,
+                      pts4 ? nullptr : f.c_dists, pts4 ? f.c_density : f.c_alpha, pts4 ? nullptr : f.c_density, s));
+  { Epi e; e.bias = c.bias(L_NF); e.out_pl = f.FEATN; NRW_TRY(mm(c, f.NH[8], c.W(L_NF), M, 256, 256, e, s)); }
   // L_NS0 is static_linear_0 of the appearance head, or views_linears.0 without it (the last layer before rgb_linear)
-  { Epi e; e.bias = c.bias(L_NS0); e.act = ACT_RELU; e.out_pl = c.AP[1]; NRW_TRY(mm(c, c.FEATN, c.W(L_NS0), M, 128, 384, e, s)); }
+  { Epi e; e.bias = c.bias(L_NS0); e.act = ACT_RELU; e.out_pl = f.AP[1]; NRW_TRY(mm(c, f.FEATN, c.W(L_NS0), M, 128, 384, e, s)); }
   const int last = c.nerf_app ? 4 : 1;
   for (int l = 1; l < last; ++l) {
-    Epi e; e.bias = c.bias(L_NS0 + l); e.act = ACT_RELU; e.out_pl = c.AP[l + 1];
-    NRW_TRY(mm(c, c.AP[l], c.W(L_NS0 + l), M, 128, 128, e, s));
+    Epi e; e.bias = c.bias(L_NS0 + l); e.act = ACT_RELU; e.out_pl = f.AP[l + 1];
+    NRW_TRY(mm(c, f.AP[l], c.W(L_NS0 + l), M, 128, 128, e, s));
   }
-  NRW_TRY(launch_head(3, c.AP[last], P, 128, M, c.f_area + c.pm.heads.nr_w, c.f_area + c.pm.heads.nr_b, ACT_NONE, nullptr,
-                      c.c_rgbbg, nullptr, s));
+  NRW_TRY(launch_head(3, f.AP[last], P, 128, M, c.f_area + c.pm.heads.nr_w, c.f_area + c.pm.heads.nr_b, ACT_NONE, nullptr,
+                      f.c_rgbbg, nullptr, s));
   return NRW_OK;
 }
 
@@ -358,38 +356,38 @@ __global__ void add_normal_grad_kernel(float* __restrict__ dn, const float* __re
 
 // d_rgb: [M,3] upstream gradient of the colour output.  Produces DFEAT (planes), c_dn (normal gradient
 // = d_nrm_comp + colour-net contribution) and accumulates per-ray appearance-code gradients.
-int color_chunk_backward(nrw_ctx& c, int M, const float* d_rgb, const float* d_nrm_comp, int rows_per_src,
-                         float* d_a_rays, int R_chunk, cudaStream_t s) {
-  c.cur_planes = c.bwd_planes > 0 ? c.bwd_planes : c.n_planes;   // 'mixed' mode: backward GEMMs in plain bf16
+int color_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_rgb, const float* d_nrm_comp,
+                         int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s) {
+  c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
   const int P = c.cur_planes;
   const Heads& H = c.pm.heads;
-  NRW_TRY(launch_head_bwd(3, c.X[4], P, 256, M, c.f_area + H.cl4_w, d_rgb, c.c_rgb, nullptr, 1, c.dX[0], nullptr,
+  NRW_TRY(launch_head_bwd(3, f.X[4], P, 256, M, c.f_area + H.cl4_w, d_rgb, f.c_rgb, nullptr, 1, c.dX[0], nullptr,
                           c.gs + H.d_cl4_w, c.gs + H.d_cl4_b, s));
   // bias gradients = column sums of each layer's pre-activation gradient; fused into the epilogue of the GEMM
   // that PRODUCES that gradient (Epi::colsum), only the head-produced one needs its own pass
   int cur = 0;
   NRW_TRY(bias_grad(c, c.dX[0], M, L_CL0 + 3, s));
   for (int l = 3; l >= 1; --l) {
-    Epi e; e.aux_relu = c.X[l].p; e.ld_relu = 256; e.out_pl = c.dX[1 - cur]; e.colsum = c.db(L_CL0 + l - 1);
-    NRW_TRY(mm_bwd(c, c.dX[cur], c.X[l], L_CL0 + l, c.dX[cur], c.WT(L_CL0 + l), M, 256, 256, e, s));
+    Epi e; e.aux_relu = f.X[l].p; e.ld_relu = 256; e.out_pl = c.dX[1 - cur]; e.colsum = c.db(L_CL0 + l - 1);
+    NRW_TRY(mm_bwd(c, c.dX[cur], f.X[l], L_CL0 + l, c.dX[cur], c.WT(L_CL0 + l), M, 256, 256, e, s));
     cur = 1 - cur;
   }
-  { Epi e; e.aux_relu = c.IN2.p; e.ld_relu = 192; e.out_pl = c.dH2; e.colsum = c.db(L_CS1);
-    NRW_TRY(mm_bwd(c, c.dX[cur], c.IN2, L_CL0, c.dX[cur], c.WT(L_CL0), M, 128, 256, e, s)); }
+  { Epi e; e.aux_relu = f.IN2.p; e.ld_relu = 192; e.out_pl = c.dH2; e.colsum = c.db(L_CS1);
+    NRW_TRY(mm_bwd(c, c.dX[cur], f.IN2, L_CL0, c.dX[cur], c.WT(L_CL0), M, 128, 256, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 64;
     NRW_TRY(mm(c, c.dX[cur], rows(c.WT(L_CL0), 128), M, 64, 256, e, s)); }
   add_normal_grad_kernel<<<cdiv(M, 256), 256, 0, s>>>(c.c_dn, d_nrm_comp, c.tail, M);
   NRW_LAUNCH_OK();
   // static_linear_1: H1 -> IN2[:, :128]
-  { Epi e; e.aux_relu = c.H1.p; e.ld_relu = 128; e.out_pl = c.dH1; e.colsum = c.db(L_CS0);
-    NRW_TRY(mm_bwd(c, c.dH2, c.H1, L_CS1, c.dH2, c.WT(L_CS1), M, 128, 128, e, s)); }
+  { Epi e; e.aux_relu = f.H1.p; e.ld_relu = 128; e.out_pl = c.dH1; e.colsum = c.db(L_CS0);
+    NRW_TRY(mm_bwd(c, c.dH2, f.H1, L_CS1, c.dH2, c.WT(L_CS1), M, 128, 128, e, s)); }
   // static_linear_0: IN1 [xf | viewPE | a] -> H1
-  { Epi e; e.out_pl = c.dXF; e.colsum = c.db(L_CX); NRW_TRY(mm_bwd(c, c.dH1, c.IN1, L_CS0, c.dH1, c.WT(L_CS0), M, 512, 128, e, s)); }
+  { Epi e; e.out_pl = c.dXF; e.colsum = c.db(L_CX); NRW_TRY(mm_bwd(c, c.dH1, f.IN1, L_CS0, c.dH1, c.WT(L_CS0), M, 512, 128, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
     NRW_TRY(mm(c, c.dH1, rows(c.WT(L_CS0), 512), M, 128, 128, e, s)); }
   if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, rows_per_src, d_a_rays, 1, s));
   // xyz_encoding_final: FEAT -> IN1[:, :512]
-  { Epi e; e.out_pl = c.DFEAT; e.colsum = c.db(L_SDF8F); NRW_TRY(mm_bwd(c, c.dXF, c.FEAT, L_CX, c.dXF, c.WT(L_CX), M, 512, 512, e, s)); }
+  { Epi e; e.out_pl = c.DFEAT; e.colsum = c.db(L_SDF8F); NRW_TRY(mm_bwd(c, c.dXF, f.FEAT, L_CX, c.dXF, c.WT(L_CX), M, 512, 512, e, s)); }
   return NRW_OK;
 }
 
@@ -400,96 +398,105 @@ static Planes dq_buf(nrw_ctx& c, int l) {
 }
 
 // d_sdf [M], c.c_dn [M,3], c.DFEAT -> parameter gradients of the SDF net (second-order backward)
-int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, cudaStream_t s) {
-  c.cur_planes = c.bwd_planes > 0 ? c.bwd_planes : c.n_planes;   // 'mixed' mode: backward GEMMs in plain bf16
+int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_sdf, cudaStream_t s) {
+  c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
   const int P = c.cur_planes;
   const Heads& H = c.pm.heads;
   const float* w0 = c.f_area + H.sdf_w0;
-  NRW_TRY(launch_sdf_normal_bwd(pts, c.c_dn, M, P, c.DQ0, c.DQ4, s));
+  NRW_TRY(launch_sdf_normal_bwd(f.PTS, c.c_dn, M, P, c.DQ0, c.DQ4, s));
   // tangent sweep: derivative of the gradient chain
   for (int l = 0; l < 8; ++l) {
     Planes DQl = dq_buf(c, l);
     Epi e;
-    gate_from(c, e, l, c.gate_planes());
-    if (l == 7) { e.aux_q = side_f32(w0, 0); e.aux_q_bcast = 1; } else { e.aux_q = c.Q[l + 1]; }
+    gate_from(f, e, l, c.bwd_gate_planes);
+    if (l == 7) { e.aux_q = side_f32(w0, 0); e.aux_q_bcast = 1; } else { e.aux_q = f.Q[l + 1]; }
     e.out2 = c.DA2[l];
     if (l == 3) { e.scale = INV_SQRT2; e.n_store = 473; }
     if (l < 7) e.out_pl = dq_buf(c, l + 1);
     else { e.out_f32 = c.DQ8f; e.ld_f32 = 512; }
     // (l = 0: the 512 x 64 weight gradient cannot pair and runs first, on its own)
-    NRW_TRY(mm_bwd(c, c.G[l], DQl, L_SDF0 + l, DQl, c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
+    NRW_TRY(mm_bwd(c, f.G[l], DQl, L_SDF0 + l, DQl, c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
   }
   NRW_TRY(launch_colsum(Planes{nullptr, 0, 0}, P, c.DQ8f, 512, M, 512, nullptr, c.gs + H.d_sdf_w0, nullptr, s));
   // reverse sweep
-  NRW_TRY(launch_colsum(c.U[8], P, nullptr, 0, M, 512, d_sdf, c.gs + H.d_sdf_w0, c.gs + H.d_sdf_b0, s));
+  NRW_TRY(launch_colsum(f.U[8], P, nullptr, 0, M, 512, d_sdf, c.gs + H.d_sdf_w0, c.gs + H.d_sdf_b0, s));
   {
     Epi e;
     e.rowvec = d_sdf; e.colvec = w0;
-    gate_from(c, e, 7, c.gate_planes());
+    gate_from(f, e, 7, c.bwd_gate_planes);
     e.aux_add = c.DA2[7];
     e.out_pl = c.DA[1];
     e.colsum = c.db(L_SDF0 + 7);
     // (db of lin8[1:] was accumulated by the colour backward)
-    NRW_TRY(mm_bwd(c, c.DFEAT, c.U[8], L_SDF8F, c.DFEAT, c.WT(L_SDF8F), M, 512, 512, e, s));
+    NRW_TRY(mm_bwd(c, c.DFEAT, f.U[8], L_SDF8F, c.DFEAT, c.WT(L_SDF8F), M, 512, 512, e, s));
   }
   for (int l = 7; l >= 1; --l) {
     Planes cur = c.DA[l & 1];
     Epi e;
-    gate_from(c, e, l - 1, c.gate_planes());
+    gate_from(f, e, l - 1, c.bwd_gate_planes);
     e.aux_add = c.DA2[l - 1];
     e.out_pl = c.DA[(l - 1) & 1];
     e.colsum = c.db(L_SDF0 + l - 1);
     if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }
-    NRW_TRY(mm_bwd(c, cur, c.U[l], L_SDF0 + l, cur, c.WT(L_SDF0 + l), M, 512, 512, e, s));
+    NRW_TRY(mm_bwd(c, cur, f.U[l], L_SDF0 + l, cur, c.WT(L_SDF0 + l), M, 512, 512, e, s));
   }
-  NRW_TRY(mm_dw(c, c.DA[0], c.U0, M, L_SDF0, s));
+  NRW_TRY(mm_dw(c, c.DA[0], f.U0, M, L_SDF0, s));
   return NRW_OK;
 }
 
-int nerf_chunk_backward(nrw_ctx& c, int M, const float* d_bga, const float* d_bgc, float* d_a_rays, int R_chunk,
-                        int T, cudaStream_t s) {
-  c.cur_planes = c.bwd_planes > 0 ? c.bwd_planes : c.n_planes;   // 'mixed' mode: backward GEMMs in plain bf16
+int nerf_chunk_backward(nrw_ctx& c, const FwdNerfSlot& f, int M, const float* d_bga, const float* d_bgc,
+                        float* d_a_rays, int R_chunk, int T, cudaStream_t s) {
+  c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
   const int P = c.cur_planes;
   const Heads& H = c.pm.heads;
   const int last = c.nerf_app ? 4 : 1;   // layers L_NS0 .. L_NS0 + last - 1 feed rgb_linear (nerf_chunk_forward)
-  NRW_TRY(launch_head_bwd(3, c.AP[last], P, 128, M, c.f_area + H.nr_w, d_bgc, nullptr, nullptr, 0, c.dNA[0], nullptr,
+  NRW_TRY(launch_head_bwd(3, f.AP[last], P, 128, M, c.f_area + H.nr_w, d_bgc, nullptr, nullptr, 0, c.dNA[0], nullptr,
                           c.gs + H.d_nr_w, c.gs + H.d_nr_b, s));
   int cur = 0;
   NRW_TRY(bias_grad(c, c.dNA[0], M, L_NS0 + last - 1, s));
   for (int l = last - 1; l >= 1; --l) {
-    Epi e; e.aux_relu = c.AP[l].p; e.ld_relu = 128; e.out_pl = c.dNA[1 - cur]; e.colsum = c.db(L_NS0 + l - 1);
-    NRW_TRY(mm_bwd(c, c.dNA[cur], c.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
+    Epi e; e.aux_relu = f.AP[l].p; e.ld_relu = 128; e.out_pl = c.dNA[1 - cur]; e.colsum = c.db(L_NS0 + l - 1);
+    NRW_TRY(mm_bwd(c, c.dNA[cur], f.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
     cur = 1 - cur;
   }
   { Epi e; e.out_pl = c.dNF; e.colsum = c.db(L_NF);
-    NRW_TRY(mm_bwd(c, c.dNA[cur], c.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
+    NRW_TRY(mm_bwd(c, c.dNA[cur], f.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
   if (c.nerf_app) {   // the appearance code's gradient: FEATN columns 283.. of L_NS0
     { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
       NRW_TRY(mm(c, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
     if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, T, d_a_rays, 1, s));
   }
   // alpha head -> d_density
-  NRW_TRY(launch_head_bwd(1, c.NH[8], P, 256, M, c.f_area + H.na_w, d_bga, c.c_density, c.c_dists, 2,
+  NRW_TRY(launch_head_bwd(1, f.NH[8], P, 256, M, c.f_area + H.na_w, d_bga, f.c_density, f.c_dists, 2,
                           Planes{nullptr, 0, 0}, c.c_ddens, c.gs + H.d_na_w, c.gs + H.d_na_b, s));
   // feature_linear: NH[8] -> FEATN[:, :256]
-  { Epi e; e.rowvec = c.c_ddens; e.colvec = c.f_area + H.na_w; e.aux_relu = c.NH[8].p; e.ld_relu = 256;
+  { Epi e; e.rowvec = c.c_ddens; e.colvec = c.f_area + H.na_w; e.aux_relu = f.NH[8].p; e.ld_relu = 256;
     e.out_pl = c.dNH[0]; e.colsum = c.db(L_N0 + 7);
-    NRW_TRY(mm_bwd(c, c.dNF, c.NH[8], L_NF, c.dNF, c.WT(L_NF), M, 256, 256, e, s)); }
+    NRW_TRY(mm_bwd(c, c.dNF, f.NH[8], L_NF, c.dNF, c.WT(L_NF), M, 256, 256, e, s)); }
   cur = 0;
   for (int l = 7; l >= 1; --l) {
-    Planes Xin = (l == 5) ? c.IN5 : c.NH[l];
+    Planes Xin = (l == 5) ? f.IN5 : f.NH[l];
     Epi e; e.aux_relu = Xin.p; e.ld_relu = Xin.ld; e.out_pl = c.dNH[1 - cur]; e.colsum = c.db(L_N0 + l - 1);
     // (the first 256 WT rows are the h part for l == 5)
     NRW_TRY(mm_bwd(c, c.dNH[cur], Xin, L_N0 + l, c.dNH[cur], c.WT(L_N0 + l), M, 256, 256, e, s));
     cur = 1 - cur;
   }
-  NRW_TRY(mm_dw(c, c.dNH[cur], c.IN0, M, L_N0, s));
+  NRW_TRY(mm_dw(c, c.dNH[cur], f.IN0, M, L_N0, s));
   return NRW_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
 // public operations
 // ---------------------------------------------------------------------------------------------
+// A point query runs its n rows [i, i + M) through slot 0 of its network's pass, chunk by chunk.  That slot may hold a
+// chunk of the last training render, so the backward of that render recomputes every chunk instead.
+template <class Slot, class F>
+static int query_chunks(nrw_ctx& c, std::vector<Slot>& slots, long long n, F&& chunk) {
+  c.fwd_cached = false;
+  for (long long i = 0; i < n; i += c.Mc) NRW_TRY(chunk(slots[0], i, (int)((n - i) < c.Mc ? (n - i) : c.Mc)));
+  return NRW_OK;
+}
+
 int sdf_query(nrw_ctx& c, const float* pts, long long n, float* sdf, cudaStream_t s) {
   if (sdf_fused_enabled(c) && n > 0) {            // no workspace, no chunking (the forward cache of a training render stays valid)
     const long long step = 1ll << 28;
@@ -497,14 +504,36 @@ int sdf_query(nrw_ctx& c, const float* pts, long long n, float* sdf, cudaStream_
       NRW_TRY(sdf_fused_query(c, pts + i * 3, (int)((n - i) < step ? (n - i) : step), sdf + i, s));
     return NRW_OK;
   }
-  c.fwd_cached = false;  // slot 0 is about to be overwritten
-  c.use_sdf_slot(0);
-  for (long long i = 0; i < n; i += c.Mc) {
-    const int M = (int)((n - i) < c.Mc ? (n - i) : c.Mc);
-    NRW_TRY(sdf_chunk_forward(c, M, pts + i * 3, false, false, s));
-    NRW_CUDA_OK(cudaMemcpyAsync(sdf + i, c.c_sdf, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
-  }
-  return NRW_OK;
+  return query_chunks(c, c.sdf_slots, n, [&](FwdSdfSlot& f, long long i, int M) -> int {
+    NRW_TRY(sdf_chunk_forward(c, f, M, pts + i * 3, false, false, s));
+    NRW_CUDA_OK(cudaMemcpyAsync(sdf + i, f.c_sdf, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
+    return NRW_OK;
+  });
+}
+
+int neuconw_query(nrw_ctx& c, const float* pts, const float* dirs, const float* a, long long n, float* rgb, float* sdf,
+                  float* normals, cudaStream_t s) {
+  return query_chunks(c, c.sdf_slots, n, [&](FwdSdfSlot& f, long long i, int M) -> int {
+    NRW_TRY(sdf_chunk_forward(c, f, M, pts + i * 3, true, rgb != nullptr, s));
+    if (rgb) {
+      NRW_TRY(color_chunk_forward(c, f, M, pts + i * 3, dirs + i * 3, a + i * c.n_a, 1, s));
+      NRW_CUDA_OK(cudaMemcpyAsync(rgb + i * 3, f.c_rgb, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
+    }
+    if (sdf) NRW_CUDA_OK(cudaMemcpyAsync(sdf + i, f.c_sdf, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
+    if (normals) NRW_CUDA_OK(cudaMemcpyAsync(normals + i * 3, f.c_nrm, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
+    return NRW_OK;
+  });
+}
+
+int nerf_query(nrw_ctx& c, const float* pts4, const float* dirs, const float* a, long long n, float* density,
+               float* rgb, cudaStream_t s) {
+  return query_chunks(c, c.nerf_slots, n, [&](FwdNerfSlot& f, long long i, int M) -> int {
+    NRW_TRY(nerf_chunk_forward(c, f, M, nullptr, dirs + i * 3, nullptr, nullptr, pts4 + i * 4,
+                               c.nerf_app ? a + i * c.n_a : nullptr, 1, 1, s));
+    NRW_CUDA_OK(cudaMemcpyAsync(density + i, f.c_density, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
+    NRW_CUDA_OK(cudaMemcpyAsync(rgb + i * 3, f.c_rgbbg, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
+    return NRW_OK;
+  });
 }
 
 int sample(nrw_ctx& c, const nrw_sampler_cfg& cfg, int R, const float* o, const float* d, const float* near,
@@ -549,55 +578,71 @@ int sample(nrw_ctx& c, const nrw_sampler_cfg& cfg, int R, const float* o, const 
   return NRW_OK;
 }
 
+// The chunks of one pass over R rays and the slots that keep their forward.  With k slots for n chunks, chunk i writes
+// slot min(i, k - 1) in the forward (visit j is chunk j), so chunks 0 .. k-2 stay resident and so does the last chunk,
+// the last one written into slot k - 1.  The backward takes chunks 0 .. k-2 from their slots, then the last chunk
+// (still in slot k - 1), then recomputes chunks k-1 .. n-2 into slot k - 1; with k >= n that is chunk order.  Without
+// `cached` the backward recomputes every chunk.
+struct ChunkVisit { int ci, slot; bool resident; };
+static ChunkVisit chunk_visit(int j, int n, int k, bool backward, bool cached) {
+  const int last = (n < k ? n : k) - 1;
+  const int ci = !backward || j < last ? j : j == last ? n - 1 : j - 1;
+  return ChunkVisit{ci, ci < last ? ci : last, backward && cached && (ci == n - 1 || ci < last)};
+}
+
+// Runs chunk(slot, resident, r0, nr, M) on every chunk of a pass in the order of chunk_visit: rays [r0, r0 + nr) of T
+// samples each, M = nr * T rows.
+template <class Slot, class F>
+static int walk_chunks(nrw_ctx& c, std::vector<Slot>& slots, int R, int T, bool backward, bool cached, F&& chunk) {
+  const int rc = c.Mc / T, n = cdiv(R, rc);
+  for (int j = 0; j < n; ++j) {
+    const ChunkVisit v = chunk_visit(j, n, (int)slots.size(), backward, cached);
+    const int r0 = v.ci * rc, nr = (R - r0) < rc ? (R - r0) : rc;
+    NRW_TRY(chunk(slots[v.slot], v.resident, r0, nr, nr * T));
+  }
+  return NRW_OK;
+}
+
+// forward of a training render's chunk, rays [r0, r0 + nr), into slot f: S samples per ray (SDF + colour) or T (NeRF)
+static int render_sdf_chunk(nrw_ctx& c, FwdSdfSlot& f, const nrw_render_io& io, int S, int r0, int nr, cudaStream_t s) {
+  NRW_TRY(launch_points(io.o + r0 * 3, io.d + r0 * 3, io.z_vals + (long long)r0 * S, io.sample_dist + r0, nr, S, 1, f.PTS, s));
+  NRW_TRY(sdf_chunk_forward(c, f, nr * S, f.PTS, true, true, s));
+  return color_chunk_forward(c, f, nr * S, f.PTS, io.d + r0 * 3, io.a_emb + (long long)r0 * c.n_a, S, s);
+}
+static int render_nerf_chunk(nrw_ctx& c, FwdNerfSlot& f, const nrw_render_io& io, int T, int r0, int nr,
+                             cudaStream_t s) {
+  return nerf_chunk_forward(c, f, nr * T, io.o + r0 * 3, io.d + r0 * 3, io.sv_z_feed + (long long)r0 * T,
+                            io.sample_dist + r0, nullptr, io.a_emb + (long long)r0 * c.n_a, T, T, s);
+}
+
 int render_forward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, cudaStream_t s) {
   const int R = cfg.R, S = cfg.S, T = cfg.S + cfg.n_outside;
   NRW_CHECK(c.bound && c.packed_valid, NRW_ERR_STATE, "render_forward: bind a workspace and pack weights first");
   NRW_CHECK(R <= c.max_rays && T <= c.max_T, NRW_ERR_WORKSPACE, "render: R=%d T=%d exceed bound workspace", R, T);
   NRW_CHECK(c.Mc >= T, NRW_ERR_WORKSPACE, "render: chunk_rows=%d smaller than one ray (%d)", c.Mc, T);
   const bool bg = cfg.n_outside > 0;
-  // chunk ci keeps its activations for the backward pass in slot min(ci, k - 1) of the k bound slots: chunks 0 .. k-2
-  // stay resident, and so does the last chunk, which is the last one written into slot k - 1 (render_backward)
   c.fwd_cached = false;
   if (bg) {
     NRW_TRY(launch_merge_sorted(R, S, cfg.n_outside, io.z_vals, io.z_out, io.sv_z_feed, s));
-    const int rc = c.Mc / T;
-    for (int r0 = 0, ci = 0; r0 < R; r0 += rc, ++ci) {
-      const int nr = (R - r0) < rc ? (R - r0) : rc;
-      const int M = nr * T;
-      c.use_nerf_slot(ci < c.n_slots_nerf ? ci : c.n_slots_nerf - 1);
-      NRW_TRY(nerf_chunk_forward(c, M, io.o + r0 * 3, io.d + r0 * 3, io.sv_z_feed + (long long)r0 * T,
-                                 io.sample_dist + r0, nullptr, io.a_emb + (long long)r0 * c.n_a, T, T, s));
-      NRW_CUDA_OK(cudaMemcpyAsync(io.sv_bg_alpha + (long long)r0 * T, c.c_alpha, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
-      NRW_CUDA_OK(cudaMemcpyAsync(io.sv_bg_rgb + (long long)r0 * T * 3, c.c_rgbbg, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
-    }
+    NRW_TRY(walk_chunks(c, c.nerf_slots, R, T, false, false, [&](FwdNerfSlot& f, bool, int r0, int nr, int M) -> int {
+      NRW_TRY(render_nerf_chunk(c, f, io, T, r0, nr, s));
+      NRW_CUDA_OK(cudaMemcpyAsync(io.sv_bg_alpha + (long long)r0 * T, f.c_alpha, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
+      NRW_CUDA_OK(cudaMemcpyAsync(io.sv_bg_rgb + (long long)r0 * T * 3, f.c_rgbbg, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
+      return NRW_OK;
+    }));
   }
-  const int rc = c.Mc / S;
-  for (int r0 = 0, ci = 0; r0 < R; r0 += rc, ++ci) {
-    const int nr = (R - r0) < rc ? (R - r0) : rc;
-    const int M = nr * S;
-    c.use_sdf_slot(ci < c.n_slots_sdf ? ci : c.n_slots_sdf - 1);
-    NRW_TRY(launch_points(io.o + r0 * 3, io.d + r0 * 3, io.z_vals + (long long)r0 * S, io.sample_dist + r0, nr, S, 1, c.PTS, s));
-    NRW_TRY(sdf_chunk_forward(c, M, c.PTS, true, true, s));
-    NRW_TRY(color_chunk_forward(c, M, c.PTS, io.d + r0 * 3, io.a_emb + (long long)r0 * c.n_a, S, s));
-    NRW_CUDA_OK(cudaMemcpyAsync(io.sv_sdf + (long long)r0 * S, c.c_sdf, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
-    NRW_CUDA_OK(cudaMemcpyAsync(io.gradients + (long long)r0 * S * 3, c.c_nrm, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
-    NRW_CUDA_OK(cudaMemcpyAsync(io.sv_rgb + (long long)r0 * S * 3, c.c_rgb, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
-  }
+  NRW_TRY(walk_chunks(c, c.sdf_slots, R, S, false, false, [&](FwdSdfSlot& f, bool, int r0, int nr, int M) -> int {
+    NRW_TRY(render_sdf_chunk(c, f, io, S, r0, nr, s));
+    NRW_CUDA_OK(cudaMemcpyAsync(io.sv_sdf + (long long)r0 * S, f.c_sdf, (size_t)M * 4, cudaMemcpyDeviceToDevice, s));
+    NRW_CUDA_OK(cudaMemcpyAsync(io.gradients + (long long)r0 * S * 3, f.c_nrm, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
+    NRW_CUDA_OK(cudaMemcpyAsync(io.sv_rgb + (long long)r0 * S * 3, f.c_rgb, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
+    return NRW_OK;
+  }));
   NRW_TRY(composite_forward(cfg, io, io.sv_sdf, io.gradients, io.sv_rgb, bg ? io.sv_bg_alpha : nullptr,
                             bg ? io.sv_bg_rgb : nullptr, c.ge_acc, s));
   c.fwd_cached = c.with_bwd;
   c.cached_R = R; c.cached_S = S; c.cached_T = T; c.cached_gen = cfg.reserved0;
   return NRW_OK;
-}
-
-// The backward visits the n chunks of a pass kept in n_slots slots (render_forward) in this order: the chunks below the
-// last slot, each from its own slot; the last chunk, which the last slot still holds; then the other chunks that shared
-// the last slot, each recomputed there.  With a slot per chunk that is chunk order.  When !cached every chunk is recomputed.
-struct ChunkWalk { int ci, slot; bool resident; };
-static ChunkWalk chunk_walk(int j, int n, int n_slots, bool cached) {
-  const int last = (n < n_slots ? n : n_slots) - 1;
-  const int ci = j < last ? j : j == last ? n - 1 : j - 1;
-  return ChunkWalk{ci, ci < last ? ci : last, cached && (ci == n - 1 || ci < last)};
 }
 
 static int backward_ready(const nrw_ctx& c, int R, int T) {
@@ -617,40 +662,20 @@ int network_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io&
   // do the slots still hold this render's forward?  Otherwise every chunk is recomputed (the generation stamp guards
   // against a second render_forward having overwritten the slots: ADVICE r1)
   const bool cached = c.fwd_cached && c.cached_R == R && c.cached_S == S && c.cached_T == T && c.cached_gen == cfg.reserved0;
-  if (bg) {
-    const int rc = c.Mc / T, n = cdiv(R, rc);
-    for (int j = 0; j < n; ++j) {
-      const ChunkWalk w = chunk_walk(j, n, c.n_slots_nerf, cached);
-      const int r0 = w.ci * rc;
-      const int nr = (R - r0) < rc ? (R - r0) : rc;
-      const int M = nr * T;
-      c.use_nerf_slot(w.slot);
-      if (!w.resident)
-        NRW_TRY(nerf_chunk_forward(c, M, io.o + r0 * 3, io.d + r0 * 3, io.sv_z_feed + (long long)r0 * T,
-                                   io.sample_dist + r0, nullptr, io.a_emb + (long long)r0 * c.n_a, T, T, s));
-      NRW_TRY(nerf_chunk_backward(c, M, d_bga + (long long)r0 * T, d_bgc + (long long)r0 * T * 3,
-                                  grad_a_emb + (long long)r0 * c.n_a, nr, T, s));
-    }
-  }
-  const int rc = c.Mc / S, n = cdiv(R, rc);
-  for (int j = 0; j < n; ++j) {
-    const ChunkWalk w = chunk_walk(j, n, c.n_slots_sdf, cached);
-    const int r0 = w.ci * rc;
-    const int nr = (R - r0) < rc ? (R - r0) : rc;
-    const int M = nr * S;
-    c.use_sdf_slot(w.slot);
-    if (!w.resident) {
-      NRW_TRY(launch_points(io.o + r0 * 3, io.d + r0 * 3, io.z_vals + (long long)r0 * S, io.sample_dist + r0, nr, S, 1, c.PTS, s));
-      NRW_TRY(sdf_chunk_forward(c, M, c.PTS, true, true, s));
-      NRW_TRY(color_chunk_forward(c, M, c.PTS, io.d + r0 * 3, io.a_emb + (long long)r0 * c.n_a, S, s));
-    }
-    NRW_TRY(color_chunk_backward(c, M, d_rgb + (long long)r0 * S * 3, d_nrm + (long long)r0 * S * 3, S,
+  if (bg)
+    NRW_TRY(walk_chunks(c, c.nerf_slots, R, T, true, cached, [&](FwdNerfSlot& f, bool resident, int r0, int nr,
+                                                                 int M) -> int {
+      if (!resident) NRW_TRY(render_nerf_chunk(c, f, io, T, r0, nr, s));
+      return nerf_chunk_backward(c, f, M, d_bga + (long long)r0 * T, d_bgc + (long long)r0 * T * 3,
+                                 grad_a_emb + (long long)r0 * c.n_a, nr, T, s);
+    }));
+  NRW_TRY(walk_chunks(c, c.sdf_slots, R, S, true, cached, [&](FwdSdfSlot& f, bool resident, int r0, int nr, int M) -> int {
+    if (!resident) NRW_TRY(render_sdf_chunk(c, f, io, S, r0, nr, s));
+    NRW_TRY(color_chunk_backward(c, f, M, d_rgb + (long long)r0 * S * 3, d_nrm + (long long)r0 * S * 3, S,
                                  grad_a_emb + (long long)r0 * c.n_a, nr, s));
-    NRW_TRY(sdf_chunk_backward(c, M, c.PTS, d_sdf + (long long)r0 * S, s));
-  }
+    return sdf_chunk_backward(c, f, M, d_sdf + (long long)r0 * S, s);
+  }));
   c.fwd_cached = false;
-  c.use_sdf_slot(0);
-  c.use_nerf_slot(0);
   return unpack_grads(c.pm, c.tab, c.params, c.packed, c.gs, grad_params, s);
 }
 

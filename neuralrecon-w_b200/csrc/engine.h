@@ -8,6 +8,8 @@
 
 // Forward activations of one chunk.  With enough HBM every chunk of a training batch
 // keeps its own slot, so the backward pass consumes them directly instead of recomputing the forward.
+// The chunk functions below work on the slot they are given; render_forward / network_backward pick it (engine.cu
+// chunk_visit), point queries use slot 0.
 struct FwdSdfSlot {
   float* PTS;
   nrw::Planes U0, U[9], G[8], FEAT;
@@ -24,31 +26,14 @@ struct FwdNerfSlot {
 
 struct nrw_ctx {
   int n_planes = 2, backend = 0, n_vocab = 0, n_a = 48;
-  int bwd_planes = 0;   // 0: same as n_planes; 1: 'mixed' precision (backward GEMMs use the hi plane only)
-  int cur_planes = 2;   // planes used by the GEMM helpers of the pass in flight
-  int bwd_gate_planes = 0;   // planes of u read for the softplus gates of the BACKWARD sweeps (0 = all forward planes)
-  int gate_planes() const { return bwd_gate_planes > 0 ? bwd_gate_planes : n_planes; }
+  int bwd_planes = 2;        // planes of the backward GEMMs: n_planes, or 1 in 'mixed' (the hi plane only)
+  int cur_planes = 2;        // planes used by the GEMM helpers of the pass in flight
+  int bwd_gate_planes = 2;   // planes of u read for the softplus gates of the backward sweeps
   int nerf_app = 1;     // 0: background NeRF without appearance head (nrw_ctx_set_nerf_appearance)
   std::vector<FwdSdfSlot> sdf_slots;
   std::vector<FwdNerfSlot> nerf_slots;
-  int n_slots_sdf = 1, n_slots_nerf = 1;
   bool fwd_cached = false;          // slots hold the forward of the last render_forward call
   int cached_R = 0, cached_S = 0, cached_T = 0, cached_gen = 0;   // gen: nrw_render_cfg::reserved0 of that call
-  void use_sdf_slot(int i) {
-    const FwdSdfSlot& s = sdf_slots[i];
-    PTS = s.PTS; U0 = s.U0; FEAT = s.FEAT; c_sdf = s.c_sdf; c_nrm = s.c_nrm; HP = s.HP;
-    for (int l = 0; l < 9; ++l) U[l] = s.U[l];
-    for (int l = 0; l < 8; ++l) { G[l] = s.G[l]; Q[l] = s.Q[l]; }
-    IN1 = s.IN1; H1 = s.H1; IN2 = s.IN2; c_rgb = s.c_rgb;
-    for (int l = 0; l < 5; ++l) X[l] = s.X[l];
-  }
-  void use_nerf_slot(int i) {
-    const FwdNerfSlot& s = nerf_slots[i];
-    IN0 = s.IN0; IN5 = s.IN5; FEATN = s.FEATN;
-    for (int l = 0; l < 9; ++l) NH[l] = s.NH[l];
-    for (int l = 0; l < 5; ++l) AP[l] = s.AP[l];
-    c_density = s.c_density; c_alpha = s.c_alpha; c_rgbbg = s.c_rgbbg; c_dists = s.c_dists;
-  }
   std::vector<nrw::ParamInfo> tab;
   nrw::PackedModel pm;
   char* packed = nullptr;
@@ -58,24 +43,14 @@ struct nrw_ctx {
   const float* params = nullptr;
   int Mc = 0, with_bwd = 0, max_rays = 0, max_T = 0;
 
-  // ---- chunk workspace (rows = Mc) ----
-  float* PTS = nullptr;
-  nrw::Planes U0, U[9], G[8], FEAT;
-  nrw::SideStream Q[8];
   bool aux_bf16 = false;     // 'mixed': Q_l (l != 0, 4) and the second-order terms DA2_l are stored as one bf16 plane
-  float* c_sdf = nullptr;
-  float* HP = nullptr;
-  float* c_nrm = nullptr;
-  nrw::Planes IN1, H1, IN2, X[5];
-  float* c_rgb = nullptr;
-  nrw::Planes IN0, NH[9], IN5, FEATN, AP[5];
-  float *c_density = nullptr, *c_alpha = nullptr, *c_rgbbg = nullptr, *c_dists = nullptr;
-  // backward
+
+  // ---- backward scratch of one chunk (rows = Mc), shared by every slot ----
   nrw::Planes DQ0, DQodd, DQeven, DQ4, DA[2], DFEAT;
   float* DQ8f = nullptr;
   nrw::SideStream DA2[8];    // second-order terms of the tangent sweep; one bf16 plane when aux_bf16
   nrw::Planes dX[2], dH2, dH1, dXF, dNA[2], dNF, dNH[2];
-  float *tail = nullptr, *c_dn = nullptr, *c_ddens = nullptr, *c_dpre3 = nullptr;
+  float *tail = nullptr, *c_dn = nullptr, *c_ddens = nullptr;
   float* gs = nullptr;       // gradient scratch (packed layout)
   float* ge_acc = nullptr;   // [2]
   // ---- per-call global arrays (rows = max_rays * max_T) ----
@@ -103,20 +78,26 @@ long long workspace_bytes(const nrw_ctx& c, int chunk_rows, int with_bwd, int ma
 int carve_workspace(nrw_ctx& c, void* base, long long bytes, int chunk_rows, int with_bwd, int max_rays,
                     int max_T, int n_slots_sdf, int n_slots_nerf, cudaStream_t s);
 
-// SDF value (+ normals, + feature planes) for M rows at positions pts [M,3]; results in c.c_sdf / c.c_nrm / c.FEAT
-int sdf_chunk_forward(nrw_ctx& c, int M, const float* pts, bool need_normal, bool need_feat, cudaStream_t s);
-int color_chunk_forward(nrw_ctx& c, int M, const float* pts, const float* dirs, const float* a, int rows_per_src,
-                        cudaStream_t s);
-int nerf_chunk_forward(nrw_ctx& c, int M, const float* o, const float* d, const float* z, const float* sdist,
-                       const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s);
-// backward of the three networks for the chunk currently resident in the workspace
-int color_chunk_backward(nrw_ctx& c, int M, const float* d_rgb, const float* d_nrm_comp, int rows_per_src,
-                         float* d_a_rays, int R_chunk, cudaStream_t s);
-int sdf_chunk_backward(nrw_ctx& c, int M, const float* pts, const float* d_sdf, cudaStream_t s);
-int nerf_chunk_backward(nrw_ctx& c, int M, const float* d_bga, const float* d_bgc, float* d_a_rays, int R_chunk,
-                        int T, cudaStream_t s);
+// SDF value (+ normals, + feature planes) for M rows at positions pts [M,3]; results in f.c_sdf / f.c_nrm / f.FEAT
+int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool need_normal, bool need_feat,
+                      cudaStream_t s);
+int color_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, const float* dirs, const float* a,
+                        int rows_per_src, cudaStream_t s);
+int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const float* d, const float* z,
+                       const float* sdist, const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s);
+// backward of the three networks for the chunk whose forward slot f holds
+int color_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_rgb, const float* d_nrm_comp,
+                         int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s);
+int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_sdf, cudaStream_t s);
+int nerf_chunk_backward(nrw_ctx& c, const FwdNerfSlot& f, int M, const float* d_bga, const float* d_bgc,
+                        float* d_a_rays, int R_chunk, int T, cudaStream_t s);
 
+// point queries of n points, in chunks of Mc rows in slot 0 of their pass (the fused SDF query uses no workspace)
 int sdf_query(nrw_ctx& c, const float* pts, long long n, float* sdf, cudaStream_t s);
+int neuconw_query(nrw_ctx& c, const float* pts, const float* dirs, const float* a, long long n, float* rgb, float* sdf,
+                  float* normals, cudaStream_t s);
+int nerf_query(nrw_ctx& c, const float* pts4, const float* dirs, const float* a, long long n, float* density,
+               float* rgb, cudaStream_t s);
 int sample(nrw_ctx& c, const nrw_sampler_cfg& cfg, int R, const float* o, const float* d, const float* near,
            const float* far, const float* s_near, const float* s_far, const float* u_ray, const float* u_out,
            float* z_vals, float* z_out, float* sample_dist, int32_t* trace_inds, int32_t* trace_order,
