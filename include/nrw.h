@@ -101,6 +101,24 @@ NRW_API int nrw_neuconw_forward(nrw_ctx* ctx, const float* pts /*[n,3]*/, const 
 /* NeRF.forward (models/nerf.py:156-182): pts4 [n,4], dirs [n,3], a [n,n_a] -> density[n], rgb[n,3] */
 NRW_API int nrw_nerf_forward(nrw_ctx* ctx, const float* pts4, const float* dirs, const float* a,
                              long long n, float* density, float* rgb, void* stream);
+/* Backward of the three queries above (models/neuconw.py:284-296, models/nerf.py:156-182): the gradients of
+ * L = <g_sdf, sdf> + <g_normals, normals> + <g_rgb, rgb> (NeuconW) or <g_density, density> + <g_rgb, rgb> (NeRF) with
+ * respect to the parameters, the points, the view directions and the appearance codes.  A NULL upstream gradient is zero
+ * and the work it would feed is skipped; a NULL output is not wanted.  grad_params (flat layout) is ACCUMULATED into, every
+ * other output is written.  The query's forward is recomputed chunk by chunk (nothing of the forward call is kept), so the
+ * gradients belong to the parameters as packed now; the SDF value is differentiated on the per-layer chain.  The normals'
+ * point gradient is a Hessian-vector product; rgb's includes the path through the normal.  Needs a workspace bound with
+ * with_backward (NRW_ERR_STATE otherwise).  NeuconW: dirs and a are needed with g_rgb.  NeRF: dirs always, a with g_rgb
+ * when the appearance head is on; grad_a from a NeRF without the appearance head is NRW_ERR_ARG.  n == 0 does nothing. */
+NRW_API int nrw_neuconw_backward(nrw_ctx* ctx, const float* pts /*[n,3]*/, const float* dirs /*[n,3] or NULL*/,
+                                 const float* a /*[n,n_a] or NULL*/, long long n, const float* g_sdf /*[n]*/,
+                                 const float* g_normals /*[n,3]*/, const float* g_rgb /*[n,3]*/, float* grad_params,
+                                 float* grad_pts /*[n,3]*/, float* grad_dirs /*[n,3]*/, float* grad_a /*[n,n_a]*/,
+                                 void* stream);
+NRW_API int nrw_nerf_backward(nrw_ctx* ctx, const float* pts4 /*[n,4]*/, const float* dirs /*[n,3]*/,
+                              const float* a /*[n,n_a] or NULL*/, long long n, const float* g_density /*[n]*/,
+                              const float* g_rgb /*[n,3]*/, float* grad_params, float* grad_pts4 /*[n,4]*/,
+                              float* grad_dirs /*[n,3]*/, float* grad_a /*[n,n_a]*/, void* stream);
 
 /* ---- NeuconWRenderer.sparse_sampler (rendering/renderer.py:458-568) ---------------------- */
 typedef struct {

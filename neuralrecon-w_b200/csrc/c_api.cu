@@ -152,6 +152,36 @@ int nrw_nerf_forward(nrw_ctx* ctx, const float* pts4, const float* dirs, const f
   NRW_GUARD_END
 }
 
+int nrw_neuconw_backward(nrw_ctx* ctx, const float* pts, const float* dirs, const float* a, long long n, const float* g_sdf,
+                         const float* g_normals, const float* g_rgb, float* grad_params, float* grad_pts, float* grad_dirs,
+                         float* grad_a, void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx != nullptr && n >= 0, NRW_ERR_ARG, "neuconw_backward: null context or n=%lld < 0", n);
+  NRW_CHECK(n == 0 || (pts && grad_params), NRW_ERR_ARG, "neuconw_backward: null pts or grad_params");
+  NRW_CHECK(!g_rgb || (dirs && a), NRW_ERR_ARG, "neuconw_backward: g_rgb needs dirs and a");
+  if (n == 0) return NRW_OK;
+  NRW_CHECK(ctx->bound && ctx->packed_valid && ctx->with_bwd, NRW_ERR_STATE,
+            "neuconw_backward: bind a workspace with backward and pack first");
+  return neuconw_query_backward(*ctx, pts, dirs, a, n, g_sdf, g_normals, g_rgb, grad_params, grad_pts, grad_dirs, grad_a,
+                                S(stream));
+  NRW_GUARD_END
+}
+
+int nrw_nerf_backward(nrw_ctx* ctx, const float* pts4, const float* dirs, const float* a, long long n, const float* g_density,
+                      const float* g_rgb, float* grad_params, float* grad_pts4, float* grad_dirs, float* grad_a,
+                      void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx != nullptr && n >= 0, NRW_ERR_ARG, "nerf_backward: null context or n=%lld < 0", n);
+  NRW_CHECK(n == 0 || (pts4 && dirs && grad_params), NRW_ERR_ARG, "nerf_backward: null pts4, dirs or grad_params");
+  NRW_CHECK(!g_rgb || !ctx->nerf_app || a, NRW_ERR_ARG, "nerf_backward: g_rgb needs a (appearance head)");
+  NRW_CHECK(!grad_a || ctx->nerf_app, NRW_ERR_ARG, "nerf_backward: grad_a requested from a NeRF without the appearance head");
+  if (n == 0) return NRW_OK;
+  NRW_CHECK(ctx->bound && ctx->packed_valid && ctx->with_bwd, NRW_ERR_STATE,
+            "nerf_backward: bind a workspace with backward and pack first");
+  return nerf_query_backward(*ctx, pts4, dirs, a, n, g_density, g_rgb, grad_params, grad_pts4, grad_dirs, grad_a, S(stream));
+  NRW_GUARD_END
+}
+
 int nrw_samples_per_ray(const nrw_sampler_cfg* cfg, int with_fine_octree) {
   const int k = cfg->up_sample_steps;
   const int n_new = (cfg->n_importance > 0 && k > 0) ? cfg->n_importance / k : 0;

@@ -314,8 +314,9 @@ int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const 
                        const float* sdist, const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s) {
   c.cur_planes = c.n_planes;
   const int P = c.n_planes;
-  // without the appearance head the code is not read: FEATN's a columns keep their zeros and meet zero weights
-  NRW_TRY(launch_nerf_embed(o, d, z, sdist, pts4, a, c.nerf_app ? c.n_a : 0, T, rows_per_src, M, P, f.IN0, f.IN5, f.FEATN,
+  // without the appearance head the code is not read: FEATN's a columns keep their zeros and meet zero weights (a
+  // query backward without a colour gradient passes no code either: the density does not read it)
+  NRW_TRY(launch_nerf_embed(o, d, z, sdist, pts4, a, c.nerf_app && a ? c.n_a : 0, T, rows_per_src, M, P, f.IN0, f.IN5, f.FEATN,
                             pts4 ? nullptr : f.c_dists, s));
   { Epi e; e.bias = c.bias(L_N0); e.act = ACT_RELU; e.out_pl = f.NH[1]; NRW_TRY(mm(c, f.IN0, c.W(L_N0), M, 256, 128, e, s)); }
   for (int l = 1; l <= 3; ++l) {
@@ -346,18 +347,25 @@ int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const 
 // ---------------------------------------------------------------------------------------------
 // backward chunks
 // ---------------------------------------------------------------------------------------------
+// dn = src (NULL: 0) + the normal columns 3..5 of the colour net's [pts | normal] gradient; d_pts (optional) = its point
+// columns 0..2
 __global__ void add_normal_grad_kernel(float* __restrict__ dn, const float* __restrict__ src,
-                                       const float* __restrict__ tail, int M) {
+                                       const float* __restrict__ tail, int M, float* __restrict__ d_pts) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
 #pragma unroll
-  for (int ch = 0; ch < 3; ++ch) dn[m * 3 + ch] = src[m * 3 + ch] + tail[(long long)m * 64 + 3 + ch];
+  for (int ch = 0; ch < 3; ++ch) {
+    dn[m * 3 + ch] = (src ? src[m * 3 + ch] : 0.0f) + tail[(long long)m * 64 + 3 + ch];
+    if (d_pts) d_pts[m * 3 + ch] = tail[(long long)m * 64 + ch];
+  }
 }
 
 // d_rgb: [M,3] upstream gradient of the colour output.  Produces DFEAT (planes), c_dn (normal gradient
-// = d_nrm_comp + colour-net contribution) and accumulates per-ray appearance-code gradients.
+// = d_nrm_comp (NULL: 0) + colour-net contribution) and accumulates per-ray appearance-code gradients.  d_pts (optional,
+// [M,3]) receives the colour net's gradient of its direct point input; c.tail keeps the view-encoding and code columns
+// of static_linear_0's input gradient ([M,128], from column 0) until the next backward call.
 int color_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_rgb, const float* d_nrm_comp,
-                         int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s) {
+                         int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s, float* d_pts) {
   c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
   const int P = c.cur_planes;
   const Heads& H = c.pm.heads;
@@ -376,7 +384,7 @@ int color_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_
     NRW_TRY(mm_bwd(c, c.dX[cur], f.IN2, L_CL0, c.dX[cur], c.WT(L_CL0), M, 128, 256, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 64;
     NRW_TRY(mm(c, c.dX[cur], rows(c.WT(L_CL0), 128), M, 64, 256, e, s)); }
-  add_normal_grad_kernel<<<cdiv(M, 256), 256, 0, s>>>(c.c_dn, d_nrm_comp, c.tail, M);
+  add_normal_grad_kernel<<<cdiv(M, 256), 256, 0, s>>>(c.c_dn, d_nrm_comp, c.tail, M, d_pts);
   NRW_LAUNCH_OK();
   // static_linear_1: H1 -> IN2[:, :128]
   { Epi e; e.aux_relu = f.H1.p; e.ld_relu = 128; e.out_pl = c.dH1; e.colsum = c.db(L_CS0);
@@ -397,13 +405,16 @@ static Planes dq_buf(nrw_ctx& c, int l) {
   return (l & 1) ? c.DQodd : c.DQeven;
 }
 
-// d_sdf [M], c.c_dn [M,3], c.DFEAT -> parameter gradients of the SDF net (second-order backward)
-int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_sdf, cudaStream_t s) {
+// d_sdf [M] (NULL: 0), c.c_dn [M,3], c.DFEAT -> parameter gradients of the SDF net (second-order backward) at the points
+// pts the slot's forward ran on.  enc_grad: also the gradient of the encoding E(pts) as the reverse sweep leaves it, in
+// c.tail [M,128]: columns 0..63 = DA_4 W_4 rows 448..511 (the skip input's E columns start at 25), 64..127 = DA_0 W_0.
+int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* pts, const float* d_sdf, bool enc_grad,
+                       cudaStream_t s) {
   c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
   const int P = c.cur_planes;
   const Heads& H = c.pm.heads;
   const float* w0 = c.f_area + H.sdf_w0;
-  NRW_TRY(launch_sdf_normal_bwd(f.PTS, c.c_dn, M, P, c.DQ0, c.DQ4, s));
+  NRW_TRY(launch_sdf_normal_bwd(pts, c.c_dn, M, P, c.DQ0, c.DQ4, s));
   // tangent sweep: derivative of the gradient chain
   for (int l = 0; l < 8; ++l) {
     Planes DQl = dq_buf(c, l);
@@ -419,10 +430,10 @@ int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_sd
   }
   NRW_TRY(launch_colsum(Planes{nullptr, 0, 0}, P, c.DQ8f, 512, M, 512, nullptr, c.gs + H.d_sdf_w0, nullptr, s));
   // reverse sweep
-  NRW_TRY(launch_colsum(f.U[8], P, nullptr, 0, M, 512, d_sdf, c.gs + H.d_sdf_w0, c.gs + H.d_sdf_b0, s));
+  if (d_sdf) NRW_TRY(launch_colsum(f.U[8], P, nullptr, 0, M, 512, d_sdf, c.gs + H.d_sdf_w0, c.gs + H.d_sdf_b0, s));
   {
     Epi e;
-    e.rowvec = d_sdf; e.colvec = w0;
+    if (d_sdf) { e.rowvec = d_sdf; e.colvec = w0; }
     gate_from(f, e, 7, c.bwd_gate_planes);
     e.aux_add = c.DA2[7];
     e.out_pl = c.DA[1];
@@ -439,49 +450,67 @@ int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_sd
     e.colsum = c.db(L_SDF0 + l - 1);
     if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }
     NRW_TRY(mm_bwd(c, cur, f.U[l], L_SDF0 + l, cur, c.WT(L_SDF0 + l), M, 512, 512, e, s));
+    if (l == 4 && enc_grad) { Epi t; t.out_f32 = c.tail; t.ld_f32 = 128; NRW_TRY(mm(c, cur, rows(c.WT(L_SDF0 + 4), 448), M, 64, 512, t, s)); }
   }
   NRW_TRY(mm_dw(c, c.DA[0], f.U0, M, L_SDF0, s));
+  if (enc_grad) { Epi t; t.out_f32 = c.tail + 64; t.ld_f32 = 128; NRW_TRY(mm(c, c.DA[0], c.WT(L_SDF0), M, 64, 512, t, s)); }
   return NRW_OK;
 }
 
 int nerf_chunk_backward(nrw_ctx& c, const FwdNerfSlot& f, int M, const float* d_bga, const float* d_bgc,
-                        float* d_a_rays, int R_chunk, int T, cudaStream_t s) {
+                        float* d_a_rays, int R_chunk, int T, cudaStream_t s, const NerfQueryGrads* q) {
   c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
   const int P = c.cur_planes;
   const Heads& H = c.pm.heads;
   const int last = c.nerf_app ? 4 : 1;   // layers L_NS0 .. L_NS0 + last - 1 feed rgb_linear (nerf_chunk_forward)
-  NRW_TRY(launch_head_bwd(3, f.AP[last], P, 128, M, c.f_area + H.nr_w, d_bgc, nullptr, nullptr, 0, c.dNA[0], nullptr,
-                          c.gs + H.d_nr_w, c.gs + H.d_nr_b, s));
+  const bool want_dirs = q && q->d_dirs;
   int cur = 0;
-  NRW_TRY(bias_grad(c, c.dNA[0], M, L_NS0 + last - 1, s));
-  for (int l = last - 1; l >= 1; --l) {
-    Epi e; e.aux_relu = f.AP[l].p; e.ld_relu = 128; e.out_pl = c.dNA[1 - cur]; e.colsum = c.db(L_NS0 + l - 1);
-    NRW_TRY(mm_bwd(c, c.dNA[cur], f.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
-    cur = 1 - cur;
+  if (d_bgc) {   // (without it c.dNF holds zeros: nerf_query_backward)
+    NRW_TRY(launch_head_bwd(3, f.AP[last], P, 128, M, c.f_area + H.nr_w, d_bgc, nullptr, nullptr, 0, c.dNA[0], nullptr,
+                            c.gs + H.d_nr_w, c.gs + H.d_nr_b, s));
+    NRW_TRY(bias_grad(c, c.dNA[0], M, L_NS0 + last - 1, s));
+    for (int l = last - 1; l >= 1; --l) {
+      Epi e; e.aux_relu = f.AP[l].p; e.ld_relu = 128; e.out_pl = c.dNA[1 - cur]; e.colsum = c.db(L_NS0 + l - 1);
+      NRW_TRY(mm_bwd(c, c.dNA[cur], f.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
+      cur = 1 - cur;
+    }
+    { Epi e; e.out_pl = c.dNF; e.colsum = c.db(L_NF);
+      NRW_TRY(mm_bwd(c, c.dNA[cur], f.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
+    if (c.nerf_app || want_dirs) {   // FEATN columns 256.. of L_NS0: view encoding 256..282, appearance code 283..
+      { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
+        NRW_TRY(mm(c, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
+      if (c.nerf_app && d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, T, d_a_rays, 1, s));
+      if (want_dirs) NRW_TRY(launch_pe_bwd(q->dirs, 3, 4, c.tail, 128, M, q->d_dirs, 0, s));
+    }
   }
-  { Epi e; e.out_pl = c.dNF; e.colsum = c.db(L_NF);
-    NRW_TRY(mm_bwd(c, c.dNA[cur], f.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
-  if (c.nerf_app) {   // the appearance code's gradient: FEATN columns 283.. of L_NS0
-    { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
-      NRW_TRY(mm(c, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
-    if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, T, d_a_rays, 1, s));
-  }
-  // alpha head -> d_density
-  NRW_TRY(launch_head_bwd(1, f.NH[8], P, 256, M, c.f_area + H.na_w, d_bga, f.c_density, f.c_dists, 2,
-                          Planes{nullptr, 0, 0}, c.c_ddens, c.gs + H.d_na_w, c.gs + H.d_na_b, s));
+  // alpha head -> d_density (a query's density output is the head's linear output itself)
+  if (d_bga)
+    NRW_TRY(launch_head_bwd(1, f.NH[8], P, 256, M, c.f_area + H.na_w, d_bga, f.c_density, q ? nullptr : f.c_dists,
+                            q ? 0 : 2, Planes{nullptr, 0, 0}, c.c_ddens, c.gs + H.d_na_w, c.gs + H.d_na_b, s));
   // feature_linear: NH[8] -> FEATN[:, :256]
-  { Epi e; e.rowvec = c.c_ddens; e.colvec = c.f_area + H.na_w; e.aux_relu = f.NH[8].p; e.ld_relu = 256;
+  { Epi e; if (d_bga) { e.rowvec = c.c_ddens; e.colvec = c.f_area + H.na_w; }
+    e.aux_relu = f.NH[8].p; e.ld_relu = 256;
     e.out_pl = c.dNH[0]; e.colsum = c.db(L_N0 + 7);
     NRW_TRY(mm_bwd(c, c.dNF, f.NH[8], L_NF, c.dNF, c.WT(L_NF), M, 256, 256, e, s)); }
   cur = 0;
+  const bool want_pts = q && q->d_pts4;
   for (int l = 7; l >= 1; --l) {
     Planes Xin = (l == 5) ? f.IN5 : f.NH[l];
+    if (l == 5 && want_pts) {   // the skip input's encoding columns IN5[:, 256:384] -> c.tail
+      Epi t; t.out_f32 = c.tail; t.ld_f32 = 128;
+      NRW_TRY(mm(c, c.dNH[cur], rows(c.WT(L_N0 + 5), 256), M, 128, 256, t, s));
+    }
     Epi e; e.aux_relu = Xin.p; e.ld_relu = Xin.ld; e.out_pl = c.dNH[1 - cur]; e.colsum = c.db(L_N0 + l - 1);
     // (the first 256 WT rows are the h part for l == 5)
     NRW_TRY(mm_bwd(c, c.dNH[cur], Xin, L_N0 + l, c.dNH[cur], c.WT(L_N0 + l), M, 256, 256, e, s));
     cur = 1 - cur;
   }
   NRW_TRY(mm_dw(c, c.dNH[cur], f.IN0, M, L_N0, s));
+  if (want_pts) {   // + the first layer's encoding gradient, then through PE10
+    Epi t; t.out_f32 = c.tail; t.ld_f32 = 128; t.atomic = 1;
+    NRW_TRY(mm(c, c.dNH[cur], c.WT(L_N0), M, 128, 256, t, s));
+    NRW_TRY(launch_pe_bwd(q->pts4, 4, 10, c.tail, 128, M, q->d_pts4, 0, s));
+  }
   return NRW_OK;
 }
 
@@ -534,6 +563,68 @@ int nerf_query(nrw_ctx& c, const float* pts4, const float* dirs, const float* a,
     NRW_CUDA_OK(cudaMemcpyAsync(rgb + i * 3, f.c_rgbbg, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
     return NRW_OK;
   });
+}
+
+// Backward of a point query.  The query saved only its inputs, so each chunk's forward is recomputed into slot 0 first
+// (the SDF value then comes from the per-layer chain, whatever the forward query used), then the chunk backward runs with
+// one row per appearance code.  Upstream gradients may be NULL (zero): the colour backward runs only with g_rgb.
+static void zero_planes(const Planes& p, int planes, int rows, cudaStream_t s, int& rc) {
+  for (int pl = 0; pl < planes && rc == NRW_OK; ++pl)
+    if (cudaMemsetAsync(p.plane(pl), 0, (size_t)rows * p.ld * 2, s) != cudaSuccess) rc = NRW_ERR_CUDA;
+}
+static int query_backward_ready(nrw_ctx& c, long long n, int n_in, float* grad_a, float* grad_dirs, bool rgb,
+                                cudaStream_t s) {
+  NRW_CHECK(c.bound && c.packed_valid && c.with_bwd, NRW_ERR_STATE, "query backward: workspace not bound for backward");
+  NRW_CUDA_OK(cudaMemsetAsync(c.gs, 0, (size_t)c.pm.grad_floats * 4, s));
+  if (grad_a) NRW_CUDA_OK(cudaMemsetAsync(grad_a, 0, (size_t)n * c.n_a * 4, s));   // accumulated per chunk (segsum)
+  if (grad_dirs && !rgb) NRW_CUDA_OK(cudaMemsetAsync(grad_dirs, 0, (size_t)n * n_in * 4, s));
+  return NRW_OK;
+}
+
+int neuconw_query_backward(nrw_ctx& c, const float* pts, const float* dirs, const float* a, long long n,
+                           const float* g_sdf, const float* g_nrm, const float* g_rgb, float* grad_params, float* grad_pts,
+                           float* grad_dirs, float* grad_a, cudaStream_t s) {
+  NRW_TRY(query_backward_ready(c, n, 3, grad_a, grad_dirs, g_rgb != nullptr, s));
+  int rc = NRW_OK;
+  if (!g_rgb) zero_planes(c.DFEAT, c.bwd_planes, c.Mc, s, rc);   // the reverse sweep's first GEMM reads DFEAT
+  NRW_TRY(rc);
+  NRW_TRY(query_chunks(c, c.sdf_slots, n, [&](FwdSdfSlot& f, long long i, int M) -> int {
+    const float* p = pts + i * 3;
+    float* gp = grad_pts ? grad_pts + i * 3 : nullptr;
+    NRW_TRY(sdf_chunk_forward(c, f, M, p, true, g_rgb != nullptr, s));
+    if (g_rgb) {
+      NRW_TRY(color_chunk_forward(c, f, M, p, dirs + i * 3, a + i * c.n_a, 1, s));
+      NRW_TRY(color_chunk_backward(c, f, M, g_rgb + i * 3, g_nrm ? g_nrm + i * 3 : nullptr, 1,
+                                   grad_a ? grad_a + i * c.n_a : nullptr, M, s, gp));
+      if (grad_dirs) NRW_TRY(launch_pe_bwd(dirs + i * 3, 3, 4, c.tail, 128, M, grad_dirs + i * 3, 0, s));
+    } else if (g_nrm) {
+      NRW_CUDA_OK(cudaMemcpyAsync(c.c_dn, g_nrm + i * 3, (size_t)M * 12, cudaMemcpyDeviceToDevice, s));
+    } else {
+      NRW_CUDA_OK(cudaMemsetAsync(c.c_dn, 0, (size_t)M * 12, s));
+    }
+    NRW_TRY(sdf_chunk_backward(c, f, M, p, g_sdf ? g_sdf + i : nullptr, gp != nullptr, s));
+    if (gp) NRW_TRY(launch_sdf_point_bwd(p, f.Q[0].f32(), f.Q[4].f32(), c.c_dn, c.tail, M, gp, g_rgb != nullptr, s));
+    return NRW_OK;
+  }));
+  return unpack_grads(c.pm, c.tab, c.params, c.packed, c.gs, grad_params, s);
+}
+
+int nerf_query_backward(nrw_ctx& c, const float* pts4, const float* dirs, const float* a, long long n,
+                        const float* g_density, const float* g_rgb, float* grad_params, float* grad_pts4,
+                        float* grad_dirs, float* grad_a, cudaStream_t s) {
+  NRW_TRY(query_backward_ready(c, n, 3, grad_a, grad_dirs, g_rgb != nullptr, s));
+  int rc = NRW_OK;
+  if (!g_rgb) zero_planes(c.dNF, c.bwd_planes, c.Mc, s, rc);      // feature_linear's data GEMM reads dNF
+  NRW_TRY(rc);
+  NRW_TRY(query_chunks(c, c.nerf_slots, n, [&](FwdNerfSlot& f, long long i, int M) -> int {
+    NRW_TRY(nerf_chunk_forward(c, f, M, nullptr, dirs + i * 3, nullptr, nullptr, pts4 + i * 4,
+                               c.nerf_app && g_rgb ? a + i * c.n_a : nullptr, 1, 1, s));
+    const NerfQueryGrads q{pts4 + i * 4, dirs + i * 3, grad_pts4 ? grad_pts4 + i * 4 : nullptr,
+                           grad_dirs ? grad_dirs + i * 3 : nullptr};
+    return nerf_chunk_backward(c, f, M, g_density ? g_density + i : nullptr, g_rgb ? g_rgb + i * 3 : nullptr,
+                               grad_a ? grad_a + i * c.n_a : nullptr, M, 1, s, &q);
+  }));
+  return unpack_grads(c.pm, c.tab, c.params, c.packed, c.gs, grad_params, s);
 }
 
 int sample(nrw_ctx& c, const nrw_sampler_cfg& cfg, int R, const float* o, const float* d, const float* near,
@@ -673,7 +764,7 @@ int network_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io&
     if (!resident) NRW_TRY(render_sdf_chunk(c, f, io, S, r0, nr, s));
     NRW_TRY(color_chunk_backward(c, f, M, d_rgb + (long long)r0 * S * 3, d_nrm + (long long)r0 * S * 3, S,
                                  grad_a_emb + (long long)r0 * c.n_a, nr, s));
-    return sdf_chunk_backward(c, f, M, d_sdf + (long long)r0 * S, s);
+    return sdf_chunk_backward(c, f, M, f.PTS, d_sdf + (long long)r0 * S, false, s);
   }));
   c.fwd_cached = false;
   return unpack_grads(c.pm, c.tab, c.params, c.packed, c.gs, grad_params, s);

@@ -87,10 +87,17 @@ int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const 
                        const float* sdist, const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s);
 // backward of the three networks for the chunk whose forward slot f holds
 int color_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_rgb, const float* d_nrm_comp,
-                         int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s);
-int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_sdf, cudaStream_t s);
+                         int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s, float* d_pts = nullptr);
+int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* pts, const float* d_sdf, bool enc_grad,
+                       cudaStream_t s);
+// A point query's NeRF inputs and the input gradients it wants (NULL: not wanted).  With it, d_bga is the gradient of the
+// density output (a training render's: of alpha), and either upstream may be NULL (zero).
+struct NerfQueryGrads {
+  const float *pts4, *dirs;
+  float *d_pts4, *d_dirs;
+};
 int nerf_chunk_backward(nrw_ctx& c, const FwdNerfSlot& f, int M, const float* d_bga, const float* d_bgc,
-                        float* d_a_rays, int R_chunk, int T, cudaStream_t s);
+                        float* d_a_rays, int R_chunk, int T, cudaStream_t s, const NerfQueryGrads* q = nullptr);
 
 // point queries of n points, in chunks of Mc rows in slot 0 of their pass (the fused SDF query uses no workspace)
 int sdf_query(nrw_ctx& c, const float* pts, long long n, float* sdf, cudaStream_t s);
@@ -98,6 +105,13 @@ int neuconw_query(nrw_ctx& c, const float* pts, const float* dirs, const float* 
                   float* normals, cudaStream_t s);
 int nerf_query(nrw_ctx& c, const float* pts4, const float* dirs, const float* a, long long n, float* density,
                float* rgb, cudaStream_t s);
+// their backward (nrw_neuconw_backward / nrw_nerf_backward): recompute each chunk's forward in slot 0, then backward
+int neuconw_query_backward(nrw_ctx& c, const float* pts, const float* dirs, const float* a, long long n,
+                           const float* g_sdf, const float* g_nrm, const float* g_rgb, float* grad_params, float* grad_pts,
+                           float* grad_dirs, float* grad_a, cudaStream_t s);
+int nerf_query_backward(nrw_ctx& c, const float* pts4, const float* dirs, const float* a, long long n,
+                        const float* g_density, const float* g_rgb, float* grad_params, float* grad_pts4,
+                        float* grad_dirs, float* grad_a, cudaStream_t s);
 int sample(nrw_ctx& c, const nrw_sampler_cfg& cfg, int R, const float* o, const float* d, const float* near,
            const float* far, const float* s_near, const float* s_far, const float* u_ray, const float* u_out,
            float* z_vals, float* z_out, float* sample_dist, int32_t* trace_inds, int32_t* trace_order,

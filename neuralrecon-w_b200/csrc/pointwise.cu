@@ -148,6 +148,74 @@ int launch_sdf_normal_bwd(const float* pts, const float* dn, int M, int n_planes
   return NRW_OK;
 }
 
+// ---- input gradients of point queries ---------------------------------------------------------------------------
+// The encodings [x, sin(f x), cos(f x)]_{f = 2^k} are separable per coordinate: coordinate c feeds column c and the
+// sin / cos columns D + 2Dk + c, D + 2Dk + D + c.  One thread per (row, coordinate).
+//
+// out[m,c] (+)= J_PE(x)^T dE:  dE[m,c] + sum_k f (cos(f x) dE[m, sin_k] - sin(f x) dE[m, cos_k])
+__global__ void pe_bwd_kernel(const float* __restrict__ x, int D, int n_freq, const float* __restrict__ dE, int ld, int M,
+                              float* __restrict__ out, int accumulate) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)M * D) return;
+  const long long m = i / D;
+  const int c = (int)(i % D);
+  const float xv = x[i];
+  const float* g = dE + m * ld;
+  float acc = g[c];
+  for (int k = 0; k < n_freq; ++k) {
+    const float f = (float)(1 << k);
+    float sn, cs;
+    sincosf(xv * f, &sn, &cs);
+    acc += f * (cs * g[D + 2 * D * k + c] - sn * g[2 * D + 2 * D * k + c]);
+  }
+  out[i] = accumulate ? out[i] + acc : acc;
+}
+int launch_pe_bwd(const float* x, int D, int n_freq, const float* dE, int ld, int M, float* out, int accumulate,
+                  cudaStream_t s) {
+  NRW_CHECK(ld >= D * (2 * n_freq + 1), NRW_ERR_ARG, "pe_bwd: ld=%d < %d encoding columns", ld, D * (2 * n_freq + 1));
+  if (M == 0) return NRW_OK;
+  pe_bwd_kernel<<<cdiv((long long)M * D, 256), 256, 0, s>>>(x, D, n_freq, dE, ld, M, out, accumulate);
+  NRW_LAUNCH_OK();
+  return NRW_OK;
+}
+
+// Point gradient of an SDF query, the mirror of sdf_normal_kernel.  With E = PE6(x):
+//   d_E = dE0[:39] + dE4[25:64] / sqrt2     (the reverse sweep's DA_0 W_0 and the skip layer's E columns of DA_4 W_4)
+//   v   = q0[:39] + q4[473:512] / sqrt2     (d sdf / d E, which the normal contracts with J_PE)
+//   out[m,c] (+)= J_PE(x)^T d_E  +  dn[m,c] sum_j v_j E_j''(x_c)     (the Hessian of E is diagonal)
+__global__ void sdf_point_bwd_kernel(const float* __restrict__ pts, const float* __restrict__ Q0, const float* __restrict__ Q4,
+                                     const float* __restrict__ dn, const float* __restrict__ dE, int M, float* __restrict__ out,
+                                     int accumulate) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)M * 3) return;
+  const long long m = i / 3;
+  const int c = (int)(i % 3);
+  const float xv = pts[i], g = dn[i];
+  const float* e0 = dE + m * 128 + 64;   // DA_0 W_0, columns 0..63
+  const float* e4 = dE + m * 128 + 25;   // DA_4 W_4 rows 448..511: the E columns 473.. start at 25
+  const float* q0 = Q0 + m * 64;
+  const float* q4 = Q4 + m * 512 + 473;
+  float acc = e0[c] + e4[c] * INV_SQRT2;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) {
+    const float f = (float)(1 << k);
+    const int js = 3 + 6 * k + c, jc = js + 3;
+    float sn, cs;
+    sincosf(xv * f, &sn, &cs);
+    const float ds = e0[js] + e4[js] * INV_SQRT2, dc = e0[jc] + e4[jc] * INV_SQRT2;
+    const float vs = q0[js] + q4[js] * INV_SQRT2, vc = q0[jc] + q4[jc] * INV_SQRT2;
+    acc += f * (cs * ds - sn * dc) - f * f * g * (sn * vs + cs * vc);
+  }
+  out[i] = accumulate ? out[i] + acc : acc;
+}
+int launch_sdf_point_bwd(const float* pts, const float* Q0, const float* Q4, const float* dn, const float* dE, int M,
+                         float* out, int accumulate, cudaStream_t s) {
+  if (M == 0) return NRW_OK;
+  sdf_point_bwd_kernel<<<cdiv((long long)M * 3, 256), 256, 0, s>>>(pts, Q0, Q4, dn, dE, M, out, accumulate);
+  NRW_LAUNCH_OK();
+  return NRW_OK;
+}
+
 // ---- narrow heads: out[m,c] = act(X[m,:] . W[c,:] + b[c]),  NOUT in {1,3} --------------------------
 // act: 0 none, 3 sigmoid.  For the NeRF alpha head (NOUT=1) `dists` turns density into
 // alpha = 1 - exp(-softplus(density) * dist) (renderer.py:205-207); density is kept in out2.

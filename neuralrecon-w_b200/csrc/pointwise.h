@@ -13,6 +13,13 @@ int launch_sdf_head_sum(const float* head_partial, int M, const float* b0, float
 int launch_sdf_normal(const float* pts, const float* Q0, const float* Q4, int M, float* nrm, cudaStream_t s);
 int launch_sdf_normal_bwd(const float* pts, const float* dn, int M, int n_planes, Planes DQ0, Planes DQ4,
                           cudaStream_t s);
+// input gradients of point queries: out [M,D] (+)= J_PE(x)^T dE for the D-coordinate encoding of n_freq frequencies whose
+// gradient dE sits in columns 0.. of rows of ld floats; the SDF query's point gradient from the tail of its reverse sweep
+// (dE: [M,128], columns 0..63 = DA_4 W_4 rows 448.., 64..127 = DA_0 W_0) and the normal's own second-derivative term
+int launch_pe_bwd(const float* x, int D, int n_freq, const float* dE, int ld, int M, float* out, int accumulate,
+                  cudaStream_t s);
+int launch_sdf_point_bwd(const float* pts, const float* Q0, const float* Q4, const float* dn, const float* dE, int M,
+                         float* out, int accumulate, cudaStream_t s);
 int launch_color_embed(const float* dirs, const float* a, int n_a, int rows_per_src, const float* pts,
                        const float* nrm, int M, int n_planes, Planes IN1, Planes IN2, cudaStream_t s);
 int launch_nerf_embed(const float* o, const float* d, const float* z, const float* sample_dist,

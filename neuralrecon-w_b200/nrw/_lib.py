@@ -93,6 +93,8 @@ def lib():
     L.nrw_sdf_query.argtypes = [vp, vp, ll, vp, vp]
     L.nrw_neuconw_forward.argtypes = [vp, vp, vp, vp, ll, vp, vp, vp, vp]
     L.nrw_nerf_forward.argtypes = [vp, vp, vp, vp, ll, vp, vp, vp]
+    L.nrw_neuconw_backward.argtypes = [vp, vp, vp, vp, ll] + [vp] * 8
+    L.nrw_nerf_backward.argtypes = [vp, vp, vp, vp, ll] + [vp] * 7
     L.nrw_sample.argtypes = [vp, C.POINTER(SamplerCfg), i32] + [vp] * 14
     L.nrw_samples_per_ray.argtypes = [C.POINTER(SamplerCfg), i32]
     L.nrw_upsample_round.argtypes = [i32, i32, i32, f32] + [vp] * 10
@@ -179,7 +181,7 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_reproject_mark", "nrw_raygen_capacity", "nrw_raygen_scratch_bytes", "nrw_raygen_image",
            "nrw_depth_range_scratch_bytes", "nrw_depth_range", "nrw_voxel_cast", "nrw_voxel_lookup",
            "nrw_view_roi_count", "nrw_label_static_count", "nrw_first_hit_scratch_bytes", "nrw_first_hit",
-           "nrw_obs_reproj_error", "nrw_ctx_set_nerf_appearance"]
+           "nrw_obs_reproj_error", "nrw_ctx_set_nerf_appearance", "nrw_neuconw_backward", "nrw_nerf_backward"]
 
 
 def check(status, what=""):

@@ -6,6 +6,7 @@ import os
 import weakref
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import NrwError, RenderCfg, RenderGrads, RenderIO, SamplerCfg, check, ptr, stream_ptr
@@ -179,8 +180,35 @@ class Engine:
         return named
 
     # ---- operations -------------------------------------------------------------------------
+    # A point query joins autograd when grad mode is on and one of its input tensors requires grad (_query_grad); the
+    # parameters then receive gradients too.  Otherwise it is the inference call below, outputs without grad_fn.
     def sdf(self, pts):
         """SDF values for pts [n,3] -> [n] (NeuconWRenderer.sdf, rendering/renderer.py:947-949)."""
+        if _query_grad(pts):
+            return _NeuconWQueryFn.apply(self, "sdf", pts, None, None, *self._query_params(pts.device))[0]
+        return self._sdf(pts)
+
+    def neuconw_forward(self, pts, dirs, a, want_rgb=True):
+        """(rgb [n,3] or None, sdf [n], normals [n,3]) of NeuconW at pts [n,3], view directions dirs [n,3] and appearance
+        codes a [n,n_a] (dirs and a are read only with want_rgb)."""
+        if _query_grad(pts, dirs if want_rgb else None, a if want_rgb else None):
+            params = self._query_params(pts.device)
+            if want_rgb:
+                return tuple(_NeuconWQueryFn.apply(self, "forward", pts, dirs, a, *params))
+            return (None, *_NeuconWQueryFn.apply(self, "gradient", pts, None, None, *params))
+        return self._neuconw_forward(pts, dirs, a, want_rgb)
+
+    def nerf_forward(self, pts4, dirs, a):
+        """(density [n,1], rgb [n,3]) of the background NeRF at pts4 [n,4], dirs [n,3], a [n,n_a] (a is not read without
+        the appearance head)."""
+        if _query_grad(pts4, dirs, a if self.nerf.encode_appearance else None):
+            return tuple(_NeRFQueryFn.apply(self, pts4, dirs, a, *self._query_params(pts4.device)))
+        return self._nerf_forward(pts4, dirs, a)
+
+    def _query_params(self, device):
+        return [p for _, p in self.flatten(device)]
+
+    def _sdf(self, pts):
         pts = pts.detach().reshape(-1, 3).contiguous().float()
         n, dev = pts.shape[0], pts.device
         self.ensure(dev, 1, 2, 0, chunk_hint=n)
@@ -189,7 +217,7 @@ class Engine:
         check(self.L.nrw_sdf_query(self.ctx, ptr(pts), pts.shape[0], ptr(out), stream_ptr()), "nrw_sdf_query")
         return out
 
-    def neuconw_forward(self, pts, dirs, a, want_rgb=True):
+    def _neuconw_forward(self, pts, dirs, a, want_rgb=True):
         pts = pts.detach().reshape(-1, 3).contiguous().float()
         n, dev = pts.shape[0], pts.device
         self.ensure(dev, 1, 2, 0, chunk_hint=n)
@@ -203,7 +231,7 @@ class Engine:
                                          stream_ptr()), "nrw_neuconw_forward")
         return rgb, sdf, nrm
 
-    def nerf_forward(self, pts4, dirs, a):
+    def _nerf_forward(self, pts4, dirs, a):
         pts4 = pts4.detach().reshape(-1, 4).contiguous().float()
         n, dev = pts4.shape[0], pts4.device
         self.ensure(dev, 1, 2, 0, chunk_hint=n)
@@ -327,6 +355,131 @@ class _RenderFn(torch.autograd.Function):
         ctx.eng = None
         pgrads = [flat_grad[off:off + numel].view(shape) for shape, off, numel in ctx.param_meta]
         return (None, None, None, None, None, None, None, g_a, g_invs.reshape(ctx.inv_s_shape), *pgrads)
+
+
+def _query_grad(*inputs):
+    """does a point query join autograd: grad mode on and some input tensor requiring grad."""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in inputs)
+
+
+def _flat(t, cols):
+    return None if t is None else t.detach().reshape(-1, cols).contiguous().float()
+
+
+def _param_grads(flat_grad, meta):
+    return [flat_grad[off:off + numel].view(shape) for shape, off, numel in meta]
+
+
+def _input_grad(g, like):
+    """a gradient in the shape and dtype of its input (like = (shape, dtype))."""
+    return None if g is None else g.view(like[0]).to(like[1])
+
+
+class _QueryFn(torch.autograd.Function):
+    """Shared plumbing of the point-query Functions.  The forward is the inference call, so its outputs equal a call under
+    no_grad.  Only the inputs are saved: the backward recomputes the query's forward chunk by chunk inside libnrw, so a
+    render or another query in between cannot leave it stale activations.  It differentiates the per-layer chain at the
+    parameters as packed when the backward runs.  Once-differentiable: differentiating the backward raises."""
+
+    @staticmethod
+    def _setup(ctx, eng, params, inputs):
+        ctx.eng = eng
+        ctx.like = [None if t is None else (t.shape, t.dtype) for t in inputs]
+        ctx.param_meta = [(p.shape, eng.index[k][1], eng.index[k][2]) for (k, _), p in zip(eng.named_params(), params)]
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def _refuse_create_graph():
+        # the backward runs with grad mode on only under create_graph=True; its result would be a constant, so a gradient
+        # of it (e.g. an eikonal term written as autograd.grad(sdf, x, create_graph=True)) would silently vanish
+        if torch.is_grad_enabled():
+            raise NrwError("NeuconW / NeRF point queries are once-differentiable: their backward cannot be differentiated "
+                           "(create_graph=True); use NeuconW.gradient(x) for the SDF's gradient")
+
+    @staticmethod
+    def _bind(eng, dev, n):
+        eng.ensure(dev, 1, 2, 1, chunk_hint=n)     # bound for backward; the ray bound does not grow
+        eng.pack(dev)
+        return torch.zeros(eng.total, dtype=torch.float32, device=dev)
+
+
+class _NeuconWQueryFn(_QueryFn):
+    """NeuconW queries: kind "sdf" -> (sdf,), "gradient" -> (sdf, normals), "forward" -> (rgb, sdf, normals)."""
+
+    @staticmethod
+    def forward(ctx, eng, kind, pts, dirs, a, *params):
+        if kind == "sdf":
+            outs = (eng._sdf(pts),)
+        else:
+            rgb, sdf, nrm = eng._neuconw_forward(pts, dirs, a, want_rgb=kind == "forward")
+            outs = (sdf, nrm) if rgb is None else (rgb, sdf, nrm)
+        ctx.kind = kind
+        _QueryFn._setup(ctx, eng, params, (pts, dirs, a))
+        ctx.save_for_backward(_flat(pts, 3), _flat(dirs, 3), None if a is None else _flat(a, eng.n_a))
+        return outs
+
+    @staticmethod
+    def backward(ctx, *grads):
+        _QueryFn._refuse_create_graph()
+        return _NeuconWQueryFn._backward(ctx, *grads)
+
+    @staticmethod
+    @once_differentiable
+    def _backward(ctx, *grads):
+        eng = ctx.eng
+        pts, dirs, a = ctx.saved_tensors
+        names = {"sdf": ("sdf",), "gradient": ("sdf", "normals"), "forward": ("rgb", "sdf", "normals")}[ctx.kind]
+        up = dict(zip(names, grads))
+        n, dev = pts.shape[0], pts.device
+        c = lambda k, cols: _flat(up.get(k), cols)
+        g_sdf, g_nrm, g_rgb = c("sdf", 1), c("normals", 3), c("rgb", 3)
+        need = ctx.needs_input_grad
+        f = lambda want, cols: torch.empty(n, cols, dtype=torch.float32, device=dev) if want else None
+        gp, gd, ga = f(need[2], 3), f(need[3], 3), f(need[4], eng.n_a)
+        flat_grad = _QueryFn._bind(eng, dev, n)
+        if n:
+            check(eng.L.nrw_neuconw_backward(eng.ctx, ptr(pts), ptr(dirs), ptr(a), n, ptr(g_sdf), ptr(g_nrm), ptr(g_rgb),
+                                             ptr(flat_grad), ptr(gp), ptr(gd), ptr(ga), stream_ptr()),
+                  "nrw_neuconw_backward")
+        x_pts, x_dirs, x_a = ctx.like
+        return (None, None, _input_grad(gp, x_pts), _input_grad(gd, x_dirs), _input_grad(ga, x_a),
+                *_param_grads(flat_grad, ctx.param_meta))
+
+
+class _NeRFQueryFn(_QueryFn):
+    """NeRF.forward: (density [n,1], rgb [n,3]).  Without the appearance head the code gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, eng, pts4, dirs, a, *params):
+        dens, rgb = eng._nerf_forward(pts4, dirs, a)
+        _QueryFn._setup(ctx, eng, params, (pts4, dirs, a))
+        app = eng.nerf.encode_appearance
+        ctx.save_for_backward(_flat(pts4, 4), _flat(dirs, 3), _flat(a, eng.n_a) if app else None)
+        return dens, rgb
+
+    @staticmethod
+    def backward(ctx, g_dens, g_rgb):
+        _QueryFn._refuse_create_graph()
+        return _NeRFQueryFn._backward(ctx, g_dens, g_rgb)
+
+    @staticmethod
+    @once_differentiable
+    def _backward(ctx, g_dens, g_rgb):
+        eng = ctx.eng
+        pts4, dirs, a = ctx.saved_tensors
+        n, dev = pts4.shape[0], pts4.device
+        need = ctx.needs_input_grad
+        f = lambda want, cols: torch.empty(n, cols, dtype=torch.float32, device=dev) if want else None
+        gp, gd = f(need[1], 4), f(need[2], 3)
+        ga = f(need[3] and a is not None, eng.n_a)
+        flat_grad = _QueryFn._bind(eng, dev, n)
+        if n:
+            check(eng.L.nrw_nerf_backward(eng.ctx, ptr(pts4), ptr(dirs), ptr(a), n, ptr(_flat(g_dens, 1)),
+                                          ptr(_flat(g_rgb, 3)), ptr(flat_grad), ptr(gp), ptr(gd), ptr(ga), stream_ptr()),
+                  "nrw_nerf_backward")
+        x_pts, x_dirs, x_a = ctx.like
+        return (None, _input_grad(gp, x_pts), _input_grad(gd, x_dirs), _input_grad(ga, x_a),
+                *_param_grads(flat_grad, ctx.param_meta))
 
 
 def make_sampler_cfg(n_samples, n_importance, up_sample_steps, n_outside, s_val_base, boundary_samples, perturb):

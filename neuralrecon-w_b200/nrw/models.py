@@ -120,8 +120,12 @@ class SingleVarianceNetwork(nn.Module):
 class NeuconW(nn.Module):
     """models/neuconw.py:299-376.  forward(x[R,S,3+3+N_A]) -> (rgb[R,S,3], inv_s[1,1], sdf[R,S], gradients[R,S,3]).
 
-    The standalone forward is inference-only (used by NeuconWRenderer.rgb / mesh colouring); the
-    differentiable training path goes through NeuconWRenderer.render."""
+    sdf, gradient and forward are differentiable when grad mode is on and an input tensor requires grad (gradient marks
+    its x, as the reference does): every parameter, the points, the view directions and the appearance codes then
+    receive gradients, computed by a CUDA backward that recomputes the query's forward.  Otherwise they are inference
+    calls whose outputs carry no grad_fn (the reference's always require grad).  The outputs are the same either way.
+    They are once-differentiable: a gradient of the gradient (create_graph=True, third order) raises.  The training path
+    goes through NeuconWRenderer.render."""
 
     def __init__(self, sdfNet_config, colorNet_config, SNet_config, in_channels_a, encode_a):
         super().__init__()
@@ -142,6 +146,7 @@ class NeuconW(nn.Module):
         return _engine_of(self, self.in_channels_a).sdf(input_xyz).reshape(-1, 1)
 
     def gradient(self, x):
+        x.requires_grad_(True)      # models/neuconw.py:285
         _, _, nrm = _engine_of(self, self.in_channels_a).neuconw_forward(x, None, None, want_rgb=False)
         return nrm
 
