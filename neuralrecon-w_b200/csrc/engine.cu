@@ -251,8 +251,10 @@ int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool n
   const float* w0 = c.f_area + c.pm.heads.sdf_w0;
   const float* b0 = c.f_area + c.pm.heads.sdf_b0;
   // forward-only query (sampler, NeuconWRenderer.sdf, mesh / refresh pipelines): the SDF head is fused into the epilogue of
-  // the last layer - u_8 is never written, the head kernel never reads it (tensor-core kernel, M >= 256)
-  const bool fused_head = !need_normal && !need_feat && M >= 256 && c.backend == NRW_GEMM_TCGEN05;
+  // the last layer - u_8 is never written, the head kernel never reads it (tensor-core kernel).  Every chunk takes this
+  // path whatever its row count, so a point's SDF does not depend on where the caller's batch splits into chunks
+  // (include/nrw.h); the epilogue stores row partials only for rows < M.
+  const bool fused_head = !need_normal && !need_feat && c.backend == NRW_GEMM_TCGEN05;
   // NRW_SDF_FUSED=1: the whole forward-only chain (encoding, 8 layers, head) as ONE kernel with the activations resident in
   // shared memory (gemm_tc.cu::sdf_fused_kernel) - two-plane operands only
   if (fused_head && sdf_fused_enabled(c)) return sdf_fused_query(c, pts, M, f.c_sdf, s);

@@ -1,6 +1,7 @@
 // Compile-time specialised epilogues of the tensor-core GEMM for the eight layer kinds that make up > 95 % of a
-// training step.  Same arithmetic, in the same order, as the runtime-parameterised epi_chunk16 (epilogue_tc.cuh) - the
-// difference is what is NOT executed: ncu's source view of the generic epilogue showed ISETP + BRA + LOP3 + IMAD + LDC
+// training step.  Same arithmetic, in the same order, as the runtime-parameterised epi_chunk16 (epilogue_tc.cuh), except
+// for the softplus gates of TANGENT and REVERSE, which epi_chunk16 forms with softplus100_d12_from_u (GATE_FWD's gate is
+// the same in both, NRW_GATE_K) - the difference is what is NOT executed: ncu's source view of the generic epilogue showed ISETP + BRA + LOP3 + IMAD + LDC
 // (flag tests, alignment checks, 64-bit address arithmetic, ReLU bit masks) at > 50 % of all issued instructions and
 // the useful FADD / FMUL / F2FP at ~12 % with the backward layers of the
 // `mixed` mode (one MMA product) bound by epilogue instruction issue, not by the tensor pipe or HBM.
@@ -57,12 +58,6 @@ inline int pick_epi_kind(const Epi& e) {
   }
   return EK_GENERIC;
 }
-
-// softplus gates from the stored softplus OUTPUT, 3 instructions: e = 2^(-100 log2(e) u) = 1 - sigmoid(100 a); s1 = 1 - e.
-// (No small-argument series and no threshold select as in softplus100_d12_from_u: the absolute error of s1 is <= 1 ulp of
-//  1.0 = 6e-8 and s2 = 100 s1 e is 2e-7 instead of exactly 0 above the softplus threshold - both far below the
-//  accumulation error of the GEMM that produced the value the gate multiplies.)
-#define NRW_GATE_K (-144.269504088896341f)   // -100 * log2(e)
 
 // Side streams of one specialised chunk in the line layout.  For a chunk pair they are loaded before the kernel's staging
 // barrier, so their latency overlaps that barrier and the other chunk's arithmetic.

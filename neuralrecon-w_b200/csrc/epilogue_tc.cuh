@@ -230,6 +230,15 @@ __device__ __forceinline__ void line_colsum_add(const float (&w)[16], int lane, 
   if ((lane & 4) == 0) atomicAdd(cs_tile + (lane & 3) * 4 + (hi16 ? 2 : 0) + (hi8 ? 1 : 0), k);   // shared-memory reduction
 }
 
+// softplus gates from the stored softplus OUTPUT, 3 instructions: e = 2^(-100 log2(e) u) = 1 - sigmoid(100 a); s1 = 1 - e.
+// (No small-argument series and no threshold select as in softplus100_d12_from_u: the absolute error of s1 is <= 1 ulp of
+//  1.0 = 6e-8 and s2 = 100 s1 e is 2e-7 instead of exactly 0 above the softplus threshold - both far below the
+//  accumulation error of the GEMM that produced the value the gate multiplies.)  GATE_FWD's gate (the normal chain of a
+// forward) is formed alike in epi_chunk16 and in the specialised kind (epilogue_fast.cuh fast_finish), so a point's
+// normal does not depend on whether its 32-row group reaches past M and takes epi_chunk16.  The backward gates of
+// epi_chunk16 (TANGENT's out2, REVERSE's aux_add) keep softplus100_d12_from_u.
+#define NRW_GATE_K (-144.269504088896341f)   // -100 * log2(e)
+
 // x_acc: the accumulator chunk (columns nc..nc+15 of rows m0w..m0w+31) in the line layout.
 // cs_tile: this CTA's shared column-sum accumulator for columns nc..nc+15 (flushed by the kernel); non-null iff e.colsum is set
 // and the epilogue is not atomic.
@@ -275,7 +284,15 @@ __device__ __forceinline__ void epi_chunk16(const Epi& e, const float (&x_acc)[1
   }
   // ---- activation / gating (elementwise, see epilogue.cuh) ----
   float w[16];
-  if (e.aux_u.p) {
+  if (e.aux_u.p && !e.out2 && !e.aux_add) {
+    // GATE_FWD's gate exactly as fast_finish forms it (u = the plain sum of the planes, the plane scale folded into the
+    // exponent's constant): a row's normal-chain value does not depend on whether its 32-row group is full
+    float u[16];
+    line_load_planes(L, e.aux_u, e.aux_u_planes, m0w, nc, n_st, 1.0f, u);
+    const float kk = NRW_GATE_K * e.aux_u_scale, sc = e.scale;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) w[i] = x[i] * fmaf(-sc, mufu_ex2(u[i] * kk), sc);
+  } else if (e.aux_u.p) {
     float a[16];   // the gate from the stored softplus OUTPUT planes (no fp32 pre-activation in HBM)
     line_load_planes(L, e.aux_u, e.aux_u_planes, m0w, nc, n_st, e.aux_u_scale, a);
     if (e.out2) {

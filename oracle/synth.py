@@ -96,7 +96,7 @@ def make_params(seed: int = 0, n_vocab: int = 5000, n_a: int = 48, jitter: float
         gain = w.norm(dim=1, keepdim=True) * (1.0 + 0.05 * jitter * torch.randn(o, 1, generator=g))
         pre = f"neuconw.color_net.lin{l}."
         P[pre + "bias"], P[pre + "weight_g"], P[pre + "weight_v"] = b, gain, w
-    for name, (o, i) in (("static_linear_0", (128, 587)), ("static_linear_1", (128, 128))):
+    for name, (o, i) in (("static_linear_0", (128, 539 + n_a)), ("static_linear_1", (128, 128))):
         w, b = _linear_default(g, o, i)
         P[f"neuconw.color_net.static_encoding.{name}.weight"] = w
         P[f"neuconw.color_net.static_encoding.{name}.bias"] = b
@@ -105,7 +105,7 @@ def make_params(seed: int = 0, n_vocab: int = 5000, n_a: int = 48, jitter: float
     for l, (o, i) in enumerate(NERF_PTS):
         w, b = _linear_default(g, o, i)
         P[f"nerf.pts_linears.{l}.weight"], P[f"nerf.pts_linears.{l}.bias"] = w, b
-    for l, (o, i) in enumerate([(128, 331), (128, 128), (128, 128), (128, 128)]):
+    for l, (o, i) in enumerate([(128, 283 + n_a), (128, 128), (128, 128), (128, 128)]):
         w, b = _linear_default(g, o, i)
         P[f"nerf.apperence_encoding.static_linear_{l}.weight"] = w
         P[f"nerf.apperence_encoding.static_linear_{l}.bias"] = b

@@ -51,35 +51,35 @@ def stream_sets(query):
     return [(k,) for k in outs] + ([outs] if len(outs) > 1 else [])
 
 
-def make_inputs(n, seed=3):
+def make_inputs(n, seed=3, n_a=N_A):
     g = torch.Generator().manual_seed(seed)
     pts = (torch.rand(n, 3, generator=g) * 2 - 1) * 0.8
     dirs = F.normalize(torch.randn(n, 3, generator=g), dim=-1)
-    a = torch.randn(n, N_A, generator=g)
+    a = torch.randn(n, n_a, generator=g)
     p = F.normalize(torch.randn(n, 3, generator=g), dim=-1) * (1.0 + 3.0 * torch.rand(n, 1, generator=g))
     r = p.norm(dim=-1, keepdim=True)
     return dict(pts=pts, dirs=dirs, a=a, pts4=torch.cat([p / r, 1.0 / r], -1))
 
 
-def params(indoor=False):
-    P = un.make_params()
+def params(indoor=False, n_a=N_A, variant=None):
+    P = un.make_params(variant, n_a)
     return {k: v for k, v in P.items() if not k.startswith(ui.APP)} if indoor else P
 
 
-def make_modules(precision, backend, indoor=False, chunk_rows=None):
+def make_modules(precision, backend, indoor=False, chunk_rows=None, n_a=N_A, variant=None):
     """NeuconW and NeRF carrying the synthetic parameters, with their Engine (held by the caller: modules keep a weak
     reference)."""
     import nrw
     from nrw.engine import Engine
 
-    P = params(indoor)
-    neuconw = nrw.NeuconW(SDF_CONFIG, COLOR_CONFIG, dict(init_val=0.3), in_channels_a=N_A, encode_a=True)
+    P = params(indoor, n_a, variant)
+    neuconw = nrw.NeuconW(SDF_CONFIG, COLOR_CONFIG, dict(init_val=0.3), in_channels_a=n_a, encode_a=True)
     nerf = nrw.NeRF(D=8, d_in=4, d_in_view=3, W=256, multires=10, multires_view=4, output_ch=4, skips=[4],
-                    encode_appearance=not indoor, in_channels_a=N_A, in_channels_dir=27, use_viewdirs=True)
+                    encode_appearance=not indoor, in_channels_a=n_a, in_channels_dir=27, use_viewdirs=True)
     neuconw.load_state_dict({k[len("neuconw."):]: v for k, v in P.items() if k.startswith("neuconw.")})
     nerf.load_state_dict({k[len("nerf."):]: v for k, v in P.items() if k.startswith("nerf.")})
     neuconw, nerf = neuconw.cuda(), nerf.cuda()
-    eng = Engine(neuconw, nerf, n_vocab=un.N_VOCAB, n_a=N_A, precision=precision, backend=backend, chunk_rows=chunk_rows)
+    eng = Engine(neuconw, nerf, n_vocab=un.N_VOCAB, n_a=n_a, precision=precision, backend=backend, chunk_rows=chunk_rows)
     return P, neuconw, nerf, eng
 
 
@@ -189,18 +189,21 @@ def cuda_grads(query, neuconw, nerf, inp, ups, st):
     return res
 
 
+def reference_case(query, n_a=N_A):
+    """(P, inputs, upstream, fp64 gradients, fp32 gradients) of the comparison at N rows."""
+    P = params(query == "nerf_indoor", n_a)
+    inp = make_inputs(N, n_a=n_a)
+    ups = make_ups(query, P, inp)
+    return P, inp, ups, reference(query, P, inp, ups, torch.float64), reference(query, P, inp, ups, torch.float32)
+
+
 @pytest.fixture(scope="module")
 def refs():
     cache = {}
 
     def get(query):
         if query not in cache:
-            indoor = query == "nerf_indoor"
-            P = params(indoor)
-            inp = make_inputs(N)
-            ups = make_ups(query, P, inp)
-            cache[query] = (P, inp, ups, reference(query, P, inp, ups, torch.float64),
-                            reference(query, P, inp, ups, torch.float32))
+            cache[query] = reference_case(query)
         return cache[query]
 
     return get
@@ -209,9 +212,14 @@ def refs():
 @pytest.mark.parametrize("mode", list(MODES))
 @pytest.mark.parametrize("query", list(QUERIES))
 def test_query_backward_vs_fp64(query, mode, refs):
-    P, inp, ups, g64, g32 = refs(query)
+    check_backward(query, mode, refs(query))
+
+
+def check_backward(query, mode, case, n_a=N_A):
+    """every parameter and input gradient of the query in `mode` against case's fp64 gradients under the rule above."""
+    P, inp, ups, g64, g32 = case
     prec, backend, pfloor, ifloor = MODES[mode]
-    _, neuconw, nerf, eng = make_modules(prec, backend, indoor=query == "nerf_indoor")
+    _, neuconw, nerf, eng = make_modules(prec, backend, indoor=query == "nerf_indoor", n_a=n_a)
     sets = stream_sets(query)
     full = g64[sets[-1]]
     fails, worst = [], {}
@@ -238,7 +246,7 @@ def test_query_backward_vs_fp64(query, mode, refs):
             if not e <= bound:
                 fails.append((tag, k, e, a, bound))
     for kind, (e, where) in sorted(worst.items()):
-        print(f"[query-bwd] {query} {mode} worst {kind} error {e:.3e} ({where})")
+        print(f"[query-bwd] {query} {mode} n_a={n_a} worst {kind} error {e:.3e} ({where})")
     assert not fails, fails[:20]
 
 

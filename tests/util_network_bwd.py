@@ -59,6 +59,9 @@ CASES = {
     "dense_bg": (24, 28, 4, None, False, "dense_bg", 14),
 }
 DENSE_BG_SHIFT = 20.03    # added to nerf.alpha_linear.bias: about half the densities exceed 20 (test_network_bwd_cpu.py)
+# subtracted from the SDF's bias: the synthetic SDF is >= 0.065 in [-1.2, 1.2]^3, and 0.3 below it has a zero level set
+# at |x| ~ 0.5 .. 0.7
+SURFACE_SHIFT = 0.3
 
 
 def geometry(name):
@@ -78,10 +81,12 @@ def stream_sets(case):
 
 
 # --------------------------------------------------------------------------------------------------- parameters
-def make_params(variant=None):
-    P = synth.make_params(seed=0, n_vocab=N_VOCAB, n_a=N_A)
+def make_params(variant=None, n_a=N_A):
+    P = synth.make_params(seed=0, n_vocab=N_VOCAB, n_a=n_a)
     if variant == "dense_bg":
         P["nerf.alpha_linear.bias"] = P["nerf.alpha_linear.bias"] + DENSE_BG_SHIFT
+    elif variant == "surface":
+        P["neuconw.sdf_net.lin8.bias"] = P["neuconw.sdf_net.lin8.bias"] - SURFACE_SHIFT * (torch.arange(513) == 0)
     else:
         assert variant is None, variant
     return P
