@@ -61,16 +61,22 @@ NRW_API int nrw_param_table(int n_vocab, int n_a, nrw_param_info* out /* host, n
 NRW_API long long nrw_param_total(int n_vocab, int n_a);
 
 /* ---- context ---------------------------------------------------------------------------
- * n_planes: bf16 operand planes per fp32 tensor (1 = bf16, 2 = bf16x3 products, 3 = bf16x6
- * products ~ fp32).  chunk_rows: samples per MLP chunk (multiple of 128). */
-NRW_API int nrw_ctx_create(nrw_ctx** out, int n_planes, int gemm_backend, int n_vocab, int n_a);
+ * precision: how every fp32 GEMM operand is split into bf16 planes (values 1..3 are the plane count).
+ *   NRW_PRECISION_BF16    forward and backward GEMMs on one bf16 plane per operand: one product per
+ *                         multiply-add, plain bf16 outputs and gradients.
+ *   NRW_PRECISION_BF16X3  forward and backward GEMMs on two planes (hi, lo): the three products
+ *                         hi.hi + hi.lo + lo.hi, accumulated in fp32.
+ *   NRW_PRECISION_BF16X6  forward and backward GEMMs on three planes: all six products of weight >= 2^-16,
+ *                         about fp32 accuracy.
+ *   NRW_PRECISION_MIXED   forward as bf16x3, so every rendered output and normal keeps split-bf16 accuracy;
+ *                         the backward GEMMs and their softplus gates read the hi plane only (bf16 gradients).
+ * Anything else is NRW_ERR_ARG.  chunk_rows: samples per MLP chunk (multiple of 128). */
+#define NRW_PRECISION_BF16 1
+#define NRW_PRECISION_BF16X3 2
+#define NRW_PRECISION_BF16X6 3
+#define NRW_PRECISION_MIXED 4
+NRW_API int nrw_ctx_create(nrw_ctx** out, int precision, int gemm_backend, int n_vocab, int n_a);
 NRW_API int nrw_ctx_destroy(nrw_ctx* ctx);
-/* mixed precision: the backward GEMMs use only the first n operand planes (0 = same as forward).  n = 1 with
- * n_planes = 2 keeps every rendered output at split-bf16 accuracy and computes gradients in plain bf16. */
-NRW_API int nrw_ctx_set_backward_planes(nrw_ctx* ctx, int n);
-/* planes of the stored softplus outputs read by the BACKWARD sweeps to rebuild the gates softplus'(a), softplus''(a)
- * (0 = all forward planes; 1 halves that stream at ~1e-3 relative gate error).  The forward gradient chain always reads all. */
-NRW_API int nrw_ctx_set_backward_gate_planes(nrw_ctx* ctx, int n);
 /* on = 0: the background NeRF has no appearance head (models/nerf.py encode_appearance=False): its colour branch is
  * relu(views_linears.0([feature, viewPE])) -> rgb_linear, the appearance code is neither read nor differentiated, and the
  * nerf.apperence_encoding.* slots of the parameter table are unused (their gradient stays 0).  Default 1.  Call before

@@ -44,18 +44,21 @@ long long nrw_param_total(int n_vocab, int n_a) {
   return tab.back().offset + round_up(tab.back().numel, 4);
 }
 
-int nrw_ctx_create(nrw_ctx** out, int n_planes, int gemm_backend, int n_vocab, int n_a) {
+int nrw_ctx_create(nrw_ctx** out, int precision, int gemm_backend, int n_vocab, int n_a) {
   NRW_GUARD_BEGIN
   NRW_CHECK(out != nullptr, NRW_ERR_ARG, "ctx_create: out is null");
-  NRW_CHECK(n_planes >= 1 && n_planes <= 3, NRW_ERR_ARG, "ctx_create: n_planes must be 1..3 (got %d)", n_planes);
+  NRW_CHECK(precision >= NRW_PRECISION_BF16 && precision <= NRW_PRECISION_MIXED, NRW_ERR_ARG,
+            "ctx_create: precision must be 1 (bf16), 2 (bf16x3), 3 (bf16x6) or 4 (mixed) (got %d)", precision);
   NRW_CHECK(gemm_backend == NRW_GEMM_TCGEN05 || gemm_backend == NRW_GEMM_SIMT, NRW_ERR_ARG, "ctx_create: backend %d", gemm_backend);
   NRW_CHECK(n_a >= 1 && n_a <= 96, NRW_ERR_ARG, "ctx_create: n_a=%d unsupported (1..96)", n_a);
   nrw_ctx* c = new (std::nothrow) nrw_ctx();
   NRW_CHECK(c != nullptr, NRW_ERR_ARG, "ctx_create: out of host memory");
-  c->n_planes = n_planes; c->backend = gemm_backend; c->n_vocab = n_vocab; c->n_a = n_a;
-  c->bwd_planes = c->bwd_gate_planes = n_planes;
+  const bool mixed = precision == NRW_PRECISION_MIXED;
+  c->n_planes = mixed ? 2 : precision;
+  c->bwd_planes = mixed ? 1 : precision;
+  c->backend = gemm_backend; c->n_vocab = n_vocab; c->n_a = n_a;
   c->tab = build_param_table(n_vocab, n_a);
-  c->pm = build_packed_model(c->tab, n_planes, true);
+  c->pm = build_packed_model(c->tab, c->n_planes, true);
   *out = c;
   return NRW_OK;
   NRW_GUARD_END
@@ -67,26 +70,6 @@ int nrw_ctx_set_nerf_appearance(nrw_ctx* ctx, int on) {
             "set_nerf_appearance: call before nrw_ctx_bind (it changes the packed layout and the workspace)");
   ctx->nerf_app = on;
   ctx->pm = build_packed_model(ctx->tab, ctx->n_planes, on != 0);
-  return NRW_OK;
-  NRW_GUARD_END
-}
-int nrw_ctx_set_backward_planes(nrw_ctx* ctx, int n) {
-  NRW_GUARD_BEGIN
-  NRW_CHECK(ctx && n >= 0 && n <= ctx->n_planes, NRW_ERR_ARG, "set_backward_planes: n=%d out of range", n);
-  NRW_CHECK(!ctx->bound, NRW_ERR_STATE, "set_backward_planes: call before nrw_ctx_bind (it changes the workspace layout)");
-  ctx->bwd_planes = n ? n : ctx->n_planes;
-  // plain-bf16 backward: the fp32 side streams only the backward pass reads (Q_l of the gradient chain, the second-order
-  // terms of the tangent sweep) are kept as ONE bf16 plane as well - their consumers multiply them into bf16 operands
-  const char* env = getenv("NRW_AUX_BF16");
-  ctx->aux_bf16 = ctx->bwd_planes == 1 && ctx->n_planes > 1 && ctx->backend == NRW_GEMM_TCGEN05 && !(env && atoi(env) == 0);
-  return NRW_OK;
-  NRW_GUARD_END
-}
-int nrw_ctx_set_backward_gate_planes(nrw_ctx* ctx, int n) {
-  NRW_GUARD_BEGIN
-  NRW_CHECK(ctx != nullptr && n >= 0 && n <= ctx->n_planes, NRW_ERR_ARG, "set_backward_gate_planes: n=%d outside 0..n_planes", n);
-  NRW_CHECK(!ctx->bound, NRW_ERR_STATE, "set_backward_gate_planes: call before nrw_ctx_bind (it changes the workspace layout)");
-  ctx->bwd_gate_planes = n ? n : ctx->n_planes;
   return NRW_OK;
   NRW_GUARD_END
 }

@@ -40,7 +40,7 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
   // In 'mixed' nothing after a chunk's own forward reads the lo plane of its activations: the backward GEMMs, gates, ReLU
   // masks and heads all run on the hi plane.  So slots 1.. keep only the hi plane of each two-plane tensor and point their
   // plane 1 (pstride = lo - hi, negative) at slot 0's lo plane, which every slot shares as scratch.
-  const bool shared_lo = P == 2 && c.bwd_planes == 1 && c.bwd_gate_planes == 1;
+  const bool shared_lo = P == 2 && c.bwd_planes == 1;
   auto fwd_planes = [&](int slot, const Planes& slot0, int ld) {
     if (slot == 0 || !shared_lo) return cv.planes(M, ld, P);
     Planes h = cv.planes(M, ld, 1);
@@ -58,7 +58,7 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
     for (int l = 0; l < 8; ++l) s.G[l] = fwd_planes(i, s0.G[l], 512);
     s.Q[0] = side_f32(cv.f32(M * 64), 64);
     for (int l = 1; l < 8; ++l)   // Q_0 and Q_4 feed the normal in fp32
-      s.Q[l] = c.aux_bf16 && l != 4 ? side_bf16(reinterpret_cast<bf16*>(cv.take(M * 512 * 2)), 512) : side_f32(cv.f32(M * 512), 512);
+      s.Q[l] = c.aux_bf16() && l != 4 ? side_bf16(reinterpret_cast<bf16*>(cv.take(M * 512 * 2)), 512) : side_f32(cv.f32(M * 512), 512);
     s.FEAT = fwd_planes(i, s0.FEAT, 512);
     s.c_sdf = cv.f32(M);
     s.HP = cv.f32(M * 8);
@@ -96,7 +96,7 @@ static void carve(nrw_ctx& c, Carver& cv, int Mc, int with_bwd, int max_rays, in
     c.DFEAT = cv.planes(M, 512, PB);
     c.DQ8f = cv.f32(M * 512);
     for (int l = 0; l < 8; ++l)
-      c.DA2[l] = c.aux_bf16 ? side_bf16(reinterpret_cast<bf16*>(cv.take(M * 512 * 2)), 512) : side_f32(cv.f32(M * 512), 512);
+      c.DA2[l] = c.aux_bf16() ? side_bf16(reinterpret_cast<bf16*>(cv.take(M * 512 * 2)), 512) : side_f32(cv.f32(M * 512), 512);
     c.dX[0] = cv.planes(M, 256, PB);
     c.dX[1] = cv.planes(M, 256, PB);
     c.dH2 = cv.planes(M, 128, PB);
@@ -157,20 +157,21 @@ int carve_workspace(nrw_ctx& c, void* base, long long bytes, int chunk_rows, int
 // ---------------------------------------------------------------------------------------------
 // GEMM helpers
 // ---------------------------------------------------------------------------------------------
-static GemmDesc mm_desc(nrw_ctx& c, Planes A, Planes B, int M, int N, int K, Epi e) {
+// P: operand planes of the pass in flight (c.n_planes in a forward chunk, c.bwd_planes in a backward chunk)
+static GemmDesc mm_desc(int P, Planes A, Planes B, int M, int N, int K, Epi e) {
   GemmDesc g;
-  g.A = A; g.B = B; g.n_planes = c.cur_planes; g.M = M; g.N = N; g.K = K; g.mn_major = 0; g.k_slices = 1;
-  if (e.out_pl.p) e.n_planes = c.cur_planes;
+  g.A = A; g.B = B; g.n_planes = P; g.M = M; g.N = N; g.K = K; g.mn_major = 0; g.k_slices = 1;
+  if (e.out_pl.p) e.n_planes = P;
   g.epi = e;
   return g;
 }
-static int mm(nrw_ctx& c, Planes A, Planes B, int M, int N, int K, Epi e, cudaStream_t s) {
-  return gemm(c.backend, mm_desc(c, A, B, M, N, K, e), s);
+static int mm(nrw_ctx& c, int P, Planes A, Planes B, int M, int N, int K, Epi e, cudaStream_t s) {
+  return gemm(c.backend, mm_desc(P, A, B, M, N, K, e), s);
 }
 // dW[layer] += dY^T X   (dY [M, Np], X [M, Kx]); atomically accumulated into the gradient scratch
-static int dw_desc(nrw_ctx& c, Planes dY, Planes X, int M, int layer, GemmDesc& g) {
+static int dw_desc(nrw_ctx& c, int P, Planes dY, Planes X, int M, int layer, GemmDesc& g) {
   const PackedLayer& L = c.pm.layers[layer];
-  g.A = dY; g.B = X; g.n_planes = c.cur_planes;
+  g.A = dY; g.B = X; g.n_planes = P;
   g.M = L.Np; g.N = L.Kp; g.K = M; g.mn_major = 1;
   Epi e;
   e.out_f32 = c.dW(layer); e.ld_f32 = L.Kp; e.atomic = 1;
@@ -191,20 +192,20 @@ static int dw_desc(nrw_ctx& c, Planes dY, Planes X, int M, int layer, GemmDesc& 
   g.k_slices = ks;
   return NRW_OK;
 }
-static int mm_dw(nrw_ctx& c, Planes dY, Planes X, int M, int layer, cudaStream_t s) {
+static int mm_dw(nrw_ctx& c, int P, Planes dY, Planes X, int M, int layer, cudaStream_t s) {
   GemmDesc g;
-  NRW_TRY(dw_desc(c, dY, X, M, layer, g));
+  NRW_TRY(dw_desc(c, P, dY, X, M, layer, g));
   return gemm(c.backend, g, s);
 }
 // A backward layer: dW[layer] += dY^T X and the data GEMM A B^T -> e, which do not read each other's outputs.  On the
 // tensor-core backend they share one launch when gemm_tc_pair_ok (NRW_BWD_PAIR=0: never); otherwise they run as two
 // launches, dW first.
-static int mm_bwd(nrw_ctx& c, Planes dY, Planes X, int layer, Planes A, Planes B, int M, int N, int K, Epi e,
+static int mm_bwd(nrw_ctx& c, int P, Planes dY, Planes X, int layer, Planes A, Planes B, int M, int N, int K, Epi e,
                   cudaStream_t s) {
   static const int pair = getenv("NRW_BWD_PAIR") ? atoi(getenv("NRW_BWD_PAIR")) : 1;
   GemmPair pr;
-  pr.data = mm_desc(c, A, B, M, N, K, e);
-  NRW_TRY(dw_desc(c, dY, X, M, layer, pr.dw));
+  pr.data = mm_desc(P, A, B, M, N, K, e);
+  NRW_TRY(dw_desc(c, P, dY, X, M, layer, pr.dw));
   if (pair && c.backend == NRW_GEMM_TCGEN05 && gemm_tc_pair_ok(pr)) {
     pr.dw.k_slices = gemm_tc_pair_k_slices(M);
     return gemm_tc_pair(pr, s);
@@ -212,8 +213,8 @@ static int mm_bwd(nrw_ctx& c, Planes dY, Planes X, int layer, Planes A, Planes B
   NRW_TRY(gemm(c.backend, pr.dw, s));
   return gemm(c.backend, pr.data, s);
 }
-static int bias_grad(nrw_ctx& c, Planes dY, int M, int layer, cudaStream_t s) {
-  return launch_colsum(dY, c.cur_planes, nullptr, 0, M, c.pm.layers[layer].Np, nullptr, c.db(layer), nullptr, s);
+static int bias_grad(nrw_ctx& c, int P, Planes dY, int M, int layer, cudaStream_t s) {
+  return launch_colsum(dY, P, nullptr, 0, M, c.pm.layers[layer].Np, nullptr, c.db(layer), nullptr, s);
 }
 // gate of SDF layer l (softplus'(a_l), softplus''(a_l)) from the planes of u_{l+1} = softplus(a_l): U[l+1] holds
 // softplus(a_l) (x 1/sqrt2 in its first 473 columns for l == 3, the skip layer's input)
@@ -245,7 +246,6 @@ static int sdf_fused_query(nrw_ctx& c, const float* pts, int M, float* sdf, cuda
 
 int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool need_normal, bool need_feat,
                       cudaStream_t s) {
-  c.cur_planes = c.n_planes;
   const int P = c.n_planes;
   NRW_TRY(launch_sdf_embed(pts, M, P, f.U0, f.U[4], s));
   const float* w0 = c.f_area + c.pm.heads.sdf_w0;
@@ -267,7 +267,7 @@ int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool n
     if (l == 7 && fused_head) { e.head_w = w0; e.head_partial = f.HP; }
     else e.out_pl = f.U[l + 1];
     if (l == 3) { e.scale = INV_SQRT2; e.n_store = 473; }
-    NRW_TRY(mm(c, l == 0 ? f.U0 : f.U[l], c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
+    NRW_TRY(mm(c, P, l == 0 ? f.U0 : f.U[l], c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
   }
   if (fused_head) NRW_TRY(launch_sdf_head_sum(f.HP, M, b0, f.c_sdf, s));
   else NRW_TRY(launch_sdf_head(f.U[8], M, w0, b0, f.c_sdf, P, need_normal ? f.G[7] : Planes{nullptr, 0, 0}, s));
@@ -275,20 +275,20 @@ int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool n
     Epi e;
     e.bias = c.bias(L_SDF8F);
     e.out_pl = f.FEAT;
-    NRW_TRY(mm(c, f.U[8], c.W(L_SDF8F), M, 512, 512, e, s));
+    NRW_TRY(mm(c, P, f.U[8], c.W(L_SDF8F), M, 512, 512, e, s));
   }
   if (need_normal) {
     for (int l = 7; l >= 1; --l) {
       Epi e;
       e.out_pre = f.Q[l];
-      gate_from(f, e, l - 1, c.n_planes);
+      gate_from(f, e, l - 1, P);
       e.out_pl = f.G[l - 1];
       if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }
-      NRW_TRY(mm(c, f.G[l], c.WT(L_SDF0 + l), M, 512, 512, e, s));
+      NRW_TRY(mm(c, P, f.G[l], c.WT(L_SDF0 + l), M, 512, 512, e, s));
     }
     Epi e;
     e.out_pre = f.Q[0];
-    NRW_TRY(mm(c, f.G[0], c.WT(L_SDF0), M, 64, 512, e, s));
+    NRW_TRY(mm(c, P, f.G[0], c.WT(L_SDF0), M, 64, 512, e, s));
     NRW_TRY(launch_sdf_normal(pts, f.Q[0].f32(), f.Q[4].f32(), M, f.c_nrm, s));
   }
   return NRW_OK;
@@ -296,16 +296,15 @@ int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool n
 
 int color_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, const float* dirs, const float* a,
                         int rows_per_src, cudaStream_t s) {
-  c.cur_planes = c.n_planes;
   const int P = c.n_planes;
   NRW_TRY(launch_color_embed(dirs, a, c.n_a, rows_per_src, pts, f.c_nrm, M, P, f.IN1, f.IN2, s));
-  { Epi e; e.bias = c.bias(L_CX); e.out_pl = f.IN1; NRW_TRY(mm(c, f.FEAT, c.W(L_CX), M, 512, 512, e, s)); }
-  { Epi e; e.bias = c.bias(L_CS0); e.act = ACT_RELU; e.out_pl = f.H1; NRW_TRY(mm(c, f.IN1, c.W(L_CS0), M, 128, 640, e, s)); }
-  { Epi e; e.bias = c.bias(L_CS1); e.act = ACT_RELU; e.out_pl = f.IN2; NRW_TRY(mm(c, f.H1, c.W(L_CS1), M, 128, 128, e, s)); }
-  { Epi e; e.bias = c.bias(L_CL0); e.act = ACT_RELU; e.out_pl = f.X[1]; NRW_TRY(mm(c, f.IN2, c.W(L_CL0), M, 256, 192, e, s)); }
+  { Epi e; e.bias = c.bias(L_CX); e.out_pl = f.IN1; NRW_TRY(mm(c, P, f.FEAT, c.W(L_CX), M, 512, 512, e, s)); }
+  { Epi e; e.bias = c.bias(L_CS0); e.act = ACT_RELU; e.out_pl = f.H1; NRW_TRY(mm(c, P, f.IN1, c.W(L_CS0), M, 128, 640, e, s)); }
+  { Epi e; e.bias = c.bias(L_CS1); e.act = ACT_RELU; e.out_pl = f.IN2; NRW_TRY(mm(c, P, f.H1, c.W(L_CS1), M, 128, 128, e, s)); }
+  { Epi e; e.bias = c.bias(L_CL0); e.act = ACT_RELU; e.out_pl = f.X[1]; NRW_TRY(mm(c, P, f.IN2, c.W(L_CL0), M, 256, 192, e, s)); }
   for (int l = 1; l <= 3; ++l) {
     Epi e; e.bias = c.bias(L_CL0 + l); e.act = ACT_RELU; e.out_pl = f.X[l + 1];
-    NRW_TRY(mm(c, f.X[l], c.W(L_CL0 + l), M, 256, 256, e, s));
+    NRW_TRY(mm(c, P, f.X[l], c.W(L_CL0 + l), M, 256, 256, e, s));
   }
   NRW_TRY(launch_head(3, f.X[4], P, 256, M, c.f_area + c.pm.heads.cl4_w, c.f_area + c.pm.heads.cl4_b, ACT_SIGMOID,
                       nullptr, f.c_rgb, nullptr, s));
@@ -314,32 +313,31 @@ int color_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, cons
 
 int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const float* d, const float* z,
                        const float* sdist, const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s) {
-  c.cur_planes = c.n_planes;
   const int P = c.n_planes;
   // without the appearance head the code is not read: FEATN's a columns keep their zeros and meet zero weights (a
   // query backward without a colour gradient passes no code either: the density does not read it)
   NRW_TRY(launch_nerf_embed(o, d, z, sdist, pts4, a, c.nerf_app && a ? c.n_a : 0, T, rows_per_src, M, P, f.IN0, f.IN5, f.FEATN,
                             pts4 ? nullptr : f.c_dists, s));
-  { Epi e; e.bias = c.bias(L_N0); e.act = ACT_RELU; e.out_pl = f.NH[1]; NRW_TRY(mm(c, f.IN0, c.W(L_N0), M, 256, 128, e, s)); }
+  { Epi e; e.bias = c.bias(L_N0); e.act = ACT_RELU; e.out_pl = f.NH[1]; NRW_TRY(mm(c, P, f.IN0, c.W(L_N0), M, 256, 128, e, s)); }
   for (int l = 1; l <= 3; ++l) {
     Epi e; e.bias = c.bias(L_N0 + l); e.act = ACT_RELU; e.out_pl = f.NH[l + 1];
-    NRW_TRY(mm(c, f.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
+    NRW_TRY(mm(c, P, f.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
   }
-  { Epi e; e.bias = c.bias(L_N0 + 4); e.act = ACT_RELU; e.out_pl = f.IN5; NRW_TRY(mm(c, f.NH[4], c.W(L_N0 + 4), M, 256, 256, e, s)); }
-  { Epi e; e.bias = c.bias(L_N0 + 5); e.act = ACT_RELU; e.out_pl = f.NH[6]; NRW_TRY(mm(c, f.IN5, c.W(L_N0 + 5), M, 256, 384, e, s)); }
+  { Epi e; e.bias = c.bias(L_N0 + 4); e.act = ACT_RELU; e.out_pl = f.IN5; NRW_TRY(mm(c, P, f.NH[4], c.W(L_N0 + 4), M, 256, 256, e, s)); }
+  { Epi e; e.bias = c.bias(L_N0 + 5); e.act = ACT_RELU; e.out_pl = f.NH[6]; NRW_TRY(mm(c, P, f.IN5, c.W(L_N0 + 5), M, 256, 384, e, s)); }
   for (int l = 6; l <= 7; ++l) {
     Epi e; e.bias = c.bias(L_N0 + l); e.act = ACT_RELU; e.out_pl = f.NH[l + 1];
-    NRW_TRY(mm(c, f.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
+    NRW_TRY(mm(c, P, f.NH[l], c.W(L_N0 + l), M, 256, 256, e, s));
   }
   NRW_TRY(launch_head(1, f.NH[8], P, 256, M, c.f_area + c.pm.heads.na_w, c.f_area + c.pm.heads.na_b, ACT_NONE,
                       pts4 ? nullptr : f.c_dists, pts4 ? f.c_density : f.c_alpha, pts4 ? nullptr : f.c_density, s));
-  { Epi e; e.bias = c.bias(L_NF); e.out_pl = f.FEATN; NRW_TRY(mm(c, f.NH[8], c.W(L_NF), M, 256, 256, e, s)); }
+  { Epi e; e.bias = c.bias(L_NF); e.out_pl = f.FEATN; NRW_TRY(mm(c, P, f.NH[8], c.W(L_NF), M, 256, 256, e, s)); }
   // L_NS0 is static_linear_0 of the appearance head, or views_linears.0 without it (the last layer before rgb_linear)
-  { Epi e; e.bias = c.bias(L_NS0); e.act = ACT_RELU; e.out_pl = f.AP[1]; NRW_TRY(mm(c, f.FEATN, c.W(L_NS0), M, 128, 384, e, s)); }
+  { Epi e; e.bias = c.bias(L_NS0); e.act = ACT_RELU; e.out_pl = f.AP[1]; NRW_TRY(mm(c, P, f.FEATN, c.W(L_NS0), M, 128, 384, e, s)); }
   const int last = c.nerf_app ? 4 : 1;
   for (int l = 1; l < last; ++l) {
     Epi e; e.bias = c.bias(L_NS0 + l); e.act = ACT_RELU; e.out_pl = f.AP[l + 1];
-    NRW_TRY(mm(c, f.AP[l], c.W(L_NS0 + l), M, 128, 128, e, s));
+    NRW_TRY(mm(c, P, f.AP[l], c.W(L_NS0 + l), M, 128, 128, e, s));
   }
   NRW_TRY(launch_head(3, f.AP[last], P, 128, M, c.f_area + c.pm.heads.nr_w, c.f_area + c.pm.heads.nr_b, ACT_NONE, nullptr,
                       f.c_rgbbg, nullptr, s));
@@ -368,36 +366,35 @@ __global__ void add_normal_grad_kernel(float* __restrict__ dn, const float* __re
 // of static_linear_0's input gradient ([M,128], from column 0) until the next backward call.
 int color_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_rgb, const float* d_nrm_comp,
                          int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s, float* d_pts) {
-  c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
-  const int P = c.cur_planes;
+  const int P = c.bwd_planes;   // 'mixed': backward GEMMs in plain bf16
   const Heads& H = c.pm.heads;
   NRW_TRY(launch_head_bwd(3, f.X[4], P, 256, M, c.f_area + H.cl4_w, d_rgb, f.c_rgb, nullptr, 1, c.dX[0], nullptr,
                           c.gs + H.d_cl4_w, c.gs + H.d_cl4_b, s));
   // bias gradients = column sums of each layer's pre-activation gradient; fused into the epilogue of the GEMM
   // that PRODUCES that gradient (Epi::colsum), only the head-produced one needs its own pass
   int cur = 0;
-  NRW_TRY(bias_grad(c, c.dX[0], M, L_CL0 + 3, s));
+  NRW_TRY(bias_grad(c, P, c.dX[0], M, L_CL0 + 3, s));
   for (int l = 3; l >= 1; --l) {
     Epi e; e.aux_relu = f.X[l].p; e.ld_relu = 256; e.out_pl = c.dX[1 - cur]; e.colsum = c.db(L_CL0 + l - 1);
-    NRW_TRY(mm_bwd(c, c.dX[cur], f.X[l], L_CL0 + l, c.dX[cur], c.WT(L_CL0 + l), M, 256, 256, e, s));
+    NRW_TRY(mm_bwd(c, P, c.dX[cur], f.X[l], L_CL0 + l, c.dX[cur], c.WT(L_CL0 + l), M, 256, 256, e, s));
     cur = 1 - cur;
   }
   { Epi e; e.aux_relu = f.IN2.p; e.ld_relu = 192; e.out_pl = c.dH2; e.colsum = c.db(L_CS1);
-    NRW_TRY(mm_bwd(c, c.dX[cur], f.IN2, L_CL0, c.dX[cur], c.WT(L_CL0), M, 128, 256, e, s)); }
+    NRW_TRY(mm_bwd(c, P, c.dX[cur], f.IN2, L_CL0, c.dX[cur], c.WT(L_CL0), M, 128, 256, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 64;
-    NRW_TRY(mm(c, c.dX[cur], rows(c.WT(L_CL0), 128), M, 64, 256, e, s)); }
+    NRW_TRY(mm(c, P, c.dX[cur], rows(c.WT(L_CL0), 128), M, 64, 256, e, s)); }
   add_normal_grad_kernel<<<cdiv(M, 256), 256, 0, s>>>(c.c_dn, d_nrm_comp, c.tail, M, d_pts);
   NRW_LAUNCH_OK();
   // static_linear_1: H1 -> IN2[:, :128]
   { Epi e; e.aux_relu = f.H1.p; e.ld_relu = 128; e.out_pl = c.dH1; e.colsum = c.db(L_CS0);
-    NRW_TRY(mm_bwd(c, c.dH2, f.H1, L_CS1, c.dH2, c.WT(L_CS1), M, 128, 128, e, s)); }
+    NRW_TRY(mm_bwd(c, P, c.dH2, f.H1, L_CS1, c.dH2, c.WT(L_CS1), M, 128, 128, e, s)); }
   // static_linear_0: IN1 [xf | viewPE | a] -> H1
-  { Epi e; e.out_pl = c.dXF; e.colsum = c.db(L_CX); NRW_TRY(mm_bwd(c, c.dH1, f.IN1, L_CS0, c.dH1, c.WT(L_CS0), M, 512, 128, e, s)); }
+  { Epi e; e.out_pl = c.dXF; e.colsum = c.db(L_CX); NRW_TRY(mm_bwd(c, P, c.dH1, f.IN1, L_CS0, c.dH1, c.WT(L_CS0), M, 512, 128, e, s)); }
   { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
-    NRW_TRY(mm(c, c.dH1, rows(c.WT(L_CS0), 512), M, 128, 128, e, s)); }
+    NRW_TRY(mm(c, P, c.dH1, rows(c.WT(L_CS0), 512), M, 128, 128, e, s)); }
   if (d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, rows_per_src, d_a_rays, 1, s));
   // xyz_encoding_final: FEAT -> IN1[:, :512]
-  { Epi e; e.out_pl = c.DFEAT; e.colsum = c.db(L_SDF8F); NRW_TRY(mm_bwd(c, c.dXF, f.FEAT, L_CX, c.dXF, c.WT(L_CX), M, 512, 512, e, s)); }
+  { Epi e; e.out_pl = c.DFEAT; e.colsum = c.db(L_SDF8F); NRW_TRY(mm_bwd(c, P, c.dXF, f.FEAT, L_CX, c.dXF, c.WT(L_CX), M, 512, 512, e, s)); }
   return NRW_OK;
 }
 
@@ -412,8 +409,7 @@ static Planes dq_buf(nrw_ctx& c, int l) {
 // c.tail [M,128]: columns 0..63 = DA_4 W_4 rows 448..511 (the skip input's E columns start at 25), 64..127 = DA_0 W_0.
 int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* pts, const float* d_sdf, bool enc_grad,
                        cudaStream_t s) {
-  c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
-  const int P = c.cur_planes;
+  const int P = c.bwd_planes;   // 'mixed': backward GEMMs in plain bf16
   const Heads& H = c.pm.heads;
   const float* w0 = c.f_area + H.sdf_w0;
   NRW_TRY(launch_sdf_normal_bwd(pts, c.c_dn, M, P, c.DQ0, c.DQ4, s));
@@ -421,14 +417,14 @@ int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* pts,
   for (int l = 0; l < 8; ++l) {
     Planes DQl = dq_buf(c, l);
     Epi e;
-    gate_from(f, e, l, c.bwd_gate_planes);
+    gate_from(f, e, l, P);
     if (l == 7) { e.aux_q = side_f32(w0, 0); e.aux_q_bcast = 1; } else { e.aux_q = f.Q[l + 1]; }
     e.out2 = c.DA2[l];
     if (l == 3) { e.scale = INV_SQRT2; e.n_store = 473; }
     if (l < 7) e.out_pl = dq_buf(c, l + 1);
     else { e.out_f32 = c.DQ8f; e.ld_f32 = 512; }
     // (l = 0: the 512 x 64 weight gradient cannot pair and runs first, on its own)
-    NRW_TRY(mm_bwd(c, f.G[l], DQl, L_SDF0 + l, DQl, c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
+    NRW_TRY(mm_bwd(c, P, f.G[l], DQl, L_SDF0 + l, DQl, c.W(L_SDF0 + l), M, 512, l == 0 ? 64 : 512, e, s));
   }
   NRW_TRY(launch_colsum(Planes{nullptr, 0, 0}, P, c.DQ8f, 512, M, 512, nullptr, c.gs + H.d_sdf_w0, nullptr, s));
   // reverse sweep
@@ -436,33 +432,32 @@ int sdf_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* pts,
   {
     Epi e;
     if (d_sdf) { e.rowvec = d_sdf; e.colvec = w0; }
-    gate_from(f, e, 7, c.bwd_gate_planes);
+    gate_from(f, e, 7, P);
     e.aux_add = c.DA2[7];
     e.out_pl = c.DA[1];
     e.colsum = c.db(L_SDF0 + 7);
     // (db of lin8[1:] was accumulated by the colour backward)
-    NRW_TRY(mm_bwd(c, c.DFEAT, f.U[8], L_SDF8F, c.DFEAT, c.WT(L_SDF8F), M, 512, 512, e, s));
+    NRW_TRY(mm_bwd(c, P, c.DFEAT, f.U[8], L_SDF8F, c.DFEAT, c.WT(L_SDF8F), M, 512, 512, e, s));
   }
   for (int l = 7; l >= 1; --l) {
     Planes cur = c.DA[l & 1];
     Epi e;
-    gate_from(f, e, l - 1, c.bwd_gate_planes);
+    gate_from(f, e, l - 1, P);
     e.aux_add = c.DA2[l - 1];
     e.out_pl = c.DA[(l - 1) & 1];
     e.colsum = c.db(L_SDF0 + l - 1);
     if (l == 4) { e.scale = INV_SQRT2; e.n_store = 473; }
-    NRW_TRY(mm_bwd(c, cur, f.U[l], L_SDF0 + l, cur, c.WT(L_SDF0 + l), M, 512, 512, e, s));
-    if (l == 4 && enc_grad) { Epi t; t.out_f32 = c.tail; t.ld_f32 = 128; NRW_TRY(mm(c, cur, rows(c.WT(L_SDF0 + 4), 448), M, 64, 512, t, s)); }
+    NRW_TRY(mm_bwd(c, P, cur, f.U[l], L_SDF0 + l, cur, c.WT(L_SDF0 + l), M, 512, 512, e, s));
+    if (l == 4 && enc_grad) { Epi t; t.out_f32 = c.tail; t.ld_f32 = 128; NRW_TRY(mm(c, P, cur, rows(c.WT(L_SDF0 + 4), 448), M, 64, 512, t, s)); }
   }
-  NRW_TRY(mm_dw(c, c.DA[0], f.U0, M, L_SDF0, s));
-  if (enc_grad) { Epi t; t.out_f32 = c.tail + 64; t.ld_f32 = 128; NRW_TRY(mm(c, c.DA[0], c.WT(L_SDF0), M, 64, 512, t, s)); }
+  NRW_TRY(mm_dw(c, P, c.DA[0], f.U0, M, L_SDF0, s));
+  if (enc_grad) { Epi t; t.out_f32 = c.tail + 64; t.ld_f32 = 128; NRW_TRY(mm(c, P, c.DA[0], c.WT(L_SDF0), M, 64, 512, t, s)); }
   return NRW_OK;
 }
 
 int nerf_chunk_backward(nrw_ctx& c, const FwdNerfSlot& f, int M, const float* d_bga, const float* d_bgc,
                         float* d_a_rays, int R_chunk, int T, cudaStream_t s, const NerfQueryGrads* q) {
-  c.cur_planes = c.bwd_planes;   // 'mixed' mode: backward GEMMs in plain bf16
-  const int P = c.cur_planes;
+  const int P = c.bwd_planes;   // 'mixed': backward GEMMs in plain bf16
   const Heads& H = c.pm.heads;
   const int last = c.nerf_app ? 4 : 1;   // layers L_NS0 .. L_NS0 + last - 1 feed rgb_linear (nerf_chunk_forward)
   const bool want_dirs = q && q->d_dirs;
@@ -470,17 +465,17 @@ int nerf_chunk_backward(nrw_ctx& c, const FwdNerfSlot& f, int M, const float* d_
   if (d_bgc) {   // (without it c.dNF holds zeros: nerf_query_backward)
     NRW_TRY(launch_head_bwd(3, f.AP[last], P, 128, M, c.f_area + H.nr_w, d_bgc, nullptr, nullptr, 0, c.dNA[0], nullptr,
                             c.gs + H.d_nr_w, c.gs + H.d_nr_b, s));
-    NRW_TRY(bias_grad(c, c.dNA[0], M, L_NS0 + last - 1, s));
+    NRW_TRY(bias_grad(c, P, c.dNA[0], M, L_NS0 + last - 1, s));
     for (int l = last - 1; l >= 1; --l) {
       Epi e; e.aux_relu = f.AP[l].p; e.ld_relu = 128; e.out_pl = c.dNA[1 - cur]; e.colsum = c.db(L_NS0 + l - 1);
-      NRW_TRY(mm_bwd(c, c.dNA[cur], f.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
+      NRW_TRY(mm_bwd(c, P, c.dNA[cur], f.AP[l], L_NS0 + l, c.dNA[cur], c.WT(L_NS0 + l), M, 128, 128, e, s));
       cur = 1 - cur;
     }
     { Epi e; e.out_pl = c.dNF; e.colsum = c.db(L_NF);
-      NRW_TRY(mm_bwd(c, c.dNA[cur], f.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
+      NRW_TRY(mm_bwd(c, P, c.dNA[cur], f.FEATN, L_NS0, c.dNA[cur], c.WT(L_NS0), M, 256, 128, e, s)); }
     if (c.nerf_app || want_dirs) {   // FEATN columns 256.. of L_NS0: view encoding 256..282, appearance code 283..
       { Epi e; e.out_f32 = c.tail; e.ld_f32 = 128;
-        NRW_TRY(mm(c, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
+        NRW_TRY(mm(c, P, c.dNA[cur], rows(c.WT(L_NS0), 256), M, 128, 128, e, s)); }
       if (c.nerf_app && d_a_rays) NRW_TRY(launch_segsum(c.tail, 128, 27, c.n_a, R_chunk, T, d_a_rays, 1, s));
       if (want_dirs) NRW_TRY(launch_pe_bwd(q->dirs, 3, 4, c.tail, 128, M, q->d_dirs, 0, s));
     }
@@ -493,24 +488,24 @@ int nerf_chunk_backward(nrw_ctx& c, const FwdNerfSlot& f, int M, const float* d_
   { Epi e; if (d_bga) { e.rowvec = c.c_ddens; e.colvec = c.f_area + H.na_w; }
     e.aux_relu = f.NH[8].p; e.ld_relu = 256;
     e.out_pl = c.dNH[0]; e.colsum = c.db(L_N0 + 7);
-    NRW_TRY(mm_bwd(c, c.dNF, f.NH[8], L_NF, c.dNF, c.WT(L_NF), M, 256, 256, e, s)); }
+    NRW_TRY(mm_bwd(c, P, c.dNF, f.NH[8], L_NF, c.dNF, c.WT(L_NF), M, 256, 256, e, s)); }
   cur = 0;
   const bool want_pts = q && q->d_pts4;
   for (int l = 7; l >= 1; --l) {
     Planes Xin = (l == 5) ? f.IN5 : f.NH[l];
     if (l == 5 && want_pts) {   // the skip input's encoding columns IN5[:, 256:384] -> c.tail
       Epi t; t.out_f32 = c.tail; t.ld_f32 = 128;
-      NRW_TRY(mm(c, c.dNH[cur], rows(c.WT(L_N0 + 5), 256), M, 128, 256, t, s));
+      NRW_TRY(mm(c, P, c.dNH[cur], rows(c.WT(L_N0 + 5), 256), M, 128, 256, t, s));
     }
     Epi e; e.aux_relu = Xin.p; e.ld_relu = Xin.ld; e.out_pl = c.dNH[1 - cur]; e.colsum = c.db(L_N0 + l - 1);
     // (the first 256 WT rows are the h part for l == 5)
-    NRW_TRY(mm_bwd(c, c.dNH[cur], Xin, L_N0 + l, c.dNH[cur], c.WT(L_N0 + l), M, 256, 256, e, s));
+    NRW_TRY(mm_bwd(c, P, c.dNH[cur], Xin, L_N0 + l, c.dNH[cur], c.WT(L_N0 + l), M, 256, 256, e, s));
     cur = 1 - cur;
   }
-  NRW_TRY(mm_dw(c, c.dNH[cur], f.IN0, M, L_N0, s));
+  NRW_TRY(mm_dw(c, P, c.dNH[cur], f.IN0, M, L_N0, s));
   if (want_pts) {   // + the first layer's encoding gradient, then through PE10
     Epi t; t.out_f32 = c.tail; t.ld_f32 = 128; t.atomic = 1;
-    NRW_TRY(mm(c, c.dNH[cur], c.WT(L_N0), M, 128, 256, t, s));
+    NRW_TRY(mm(c, P, c.dNH[cur], c.WT(L_N0), M, 128, 256, t, s));
     NRW_TRY(launch_pe_bwd(q->pts4, 4, 10, c.tail, 128, M, q->d_pts4, 0, s));
   }
   return NRW_OK;

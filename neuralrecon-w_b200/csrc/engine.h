@@ -26,9 +26,7 @@ struct FwdNerfSlot {
 
 struct nrw_ctx {
   int n_planes = 2, backend = 0, n_vocab = 0, n_a = 48;
-  int bwd_planes = 2;        // planes of the backward GEMMs: n_planes, or 1 in 'mixed' (the hi plane only)
-  int cur_planes = 2;        // planes used by the GEMM helpers of the pass in flight
-  int bwd_gate_planes = 2;   // planes of u read for the softplus gates of the backward sweeps
+  int bwd_planes = 2;   // planes of the backward GEMMs and of u for their softplus gates: n_planes, or 1 in 'mixed'
   int nerf_app = 1;     // 0: background NeRF without appearance head (nrw_ctx_set_nerf_appearance)
   std::vector<FwdSdfSlot> sdf_slots;
   std::vector<FwdNerfSlot> nerf_slots;
@@ -43,7 +41,9 @@ struct nrw_ctx {
   const float* params = nullptr;
   int Mc = 0, with_bwd = 0, max_rays = 0, max_T = 0;
 
-  bool aux_bf16 = false;     // 'mixed': Q_l (l != 0, 4) and the second-order terms DA2_l are stored as one bf16 plane
+  // 'mixed' on the tensor cores: Q_l (l != 0, 4) and the second-order terms DA2_l are stored as one bf16 plane
+  // (gemm_simt takes fp32 side streams only)
+  bool aux_bf16() const { return n_planes == 2 && bwd_planes == 1 && backend == NRW_GEMM_TCGEN05; }
 
   // ---- backward scratch of one chunk (rows = Mc), shared by every slot ----
   nrw::Planes DQ0, DQodd, DQeven, DQ4, DA[2], DFEAT;

@@ -9,6 +9,11 @@ LIB_PATH = os.environ.get("NRW_LIB_PATH") or os.path.join(_HERE, "libnrw.so")   
 NRW_GEMM_TCGEN05 = 0
 NRW_GEMM_SIMT = 1
 
+NRW_PRECISION_BF16 = 1
+NRW_PRECISION_BF16X3 = 2
+NRW_PRECISION_BF16X6 = 3
+NRW_PRECISION_MIXED = 4
+
 
 class NrwError(RuntimeError):
     pass
@@ -81,8 +86,6 @@ def lib():
     L.nrw_param_total.argtypes = [i32, i32]
     L.nrw_ctx_create.argtypes = [C.POINTER(vp), i32, i32, i32, i32]
     L.nrw_ctx_destroy.argtypes = [vp]
-    L.nrw_ctx_set_backward_planes.argtypes = [vp, i32]
-    L.nrw_ctx_set_backward_gate_planes.argtypes = [vp, i32]
     L.nrw_ctx_set_nerf_appearance.argtypes = [vp, i32]
     L.nrw_packed_bytes.restype = ll
     L.nrw_packed_bytes.argtypes = [vp]
@@ -172,9 +175,9 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_composite_forward", "nrw_composite_backward", "nrw_network_backward", "nrw_octree_near_far",
            "nrw_octree_hits",
            "nrw_gemm_test_scratch_bytes", "nrw_gemm_test", "nrw_gemm_pair_test", "nrw_launch_count", "nrw_debug_gemm_profile",
-           "nrw_gemm_timing", "nrw_ctx_set_backward_planes", "nrw_octree_build_scratch_bytes", "nrw_octree_build",
+           "nrw_gemm_timing", "nrw_octree_build_scratch_bytes", "nrw_octree_build",
            "nrw_grad_sumsq", "nrw_adam_clip_step", "nrw_boundary_samples", "nrw_compact_scratch_bytes", "nrw_raycache_gather",
-           "nrw_grid_points_dense", "nrw_grid_points_sparse", "nrw_threshold_compact", "nrw_ctx_set_backward_gate_planes",
+           "nrw_grid_points_dense", "nrw_grid_points_sparse", "nrw_threshold_compact",
            "nrw_mc_scratch_bytes", "nrw_mc_count", "nrw_mc_emit",
            "nrw_nn_index_bytes", "nrw_nn_build", "nrw_nn_query_scratch_bytes", "nrw_nn_query", "nrw_mesh_sample_scratch_bytes",
            "nrw_mesh_sample", "nrw_raster_scratch_bytes", "nrw_raster_depth", "nrw_reproject_scratch_bytes",

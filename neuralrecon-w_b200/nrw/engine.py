@@ -11,8 +11,9 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 from ._lib import NrwError, RenderCfg, RenderGrads, RenderIO, SamplerCfg, check, ptr, stream_ptr
 
-# name -> (forward planes, backward planes; 0 = same).  "mixed": bf16x3 forward, plain bf16 backward GEMMs.
-PRECISIONS = {"bf16": (1, 0), "bf16x3": (2, 0), "bf16x6": (3, 0), "mixed": (2, 1)}
+# name -> nrw_ctx_create precision (include/nrw.h).  "mixed": bf16x3 forward, plain bf16 backward GEMMs.
+PRECISIONS = {"bf16": _lib.NRW_PRECISION_BF16, "bf16x3": _lib.NRW_PRECISION_BF16X3, "bf16x6": _lib.NRW_PRECISION_BF16X6,
+              "mixed": _lib.NRW_PRECISION_MIXED}
 
 
 def default_precision():
@@ -37,23 +38,15 @@ class Engine:
         self.precision = precision or default_precision()
         if self.precision not in PRECISIONS:
             raise NrwError(f"unknown precision {self.precision!r}; choose from {sorted(PRECISIONS)}")
-        self.n_planes, self.bwd_planes = PRECISIONS[self.precision]
         self.backend = default_backend() if backend is None else backend
         self.chunk_rows = int(chunk_rows or os.environ.get("NRW_CHUNK_ROWS", 262144))
         self.table, self.total = _lib.param_table(self.n_vocab, self.n_a)
         self.index = {name: (shape, off, numel) for name, shape, off, numel in self.table}
         self.ctx = C.c_void_p()
-        check(self.L.nrw_ctx_create(C.byref(self.ctx), self.n_planes, self.backend, self.n_vocab, self.n_a),
+        check(self.L.nrw_ctx_create(C.byref(self.ctx), PRECISIONS[self.precision], self.backend, self.n_vocab, self.n_a),
               "nrw_ctx_create")
         if nerf is not None and not nerf.encode_appearance:
             check(self.L.nrw_ctx_set_nerf_appearance(self.ctx, 0), "nrw_ctx_set_nerf_appearance")
-        if self.bwd_planes:
-            check(self.L.nrw_ctx_set_backward_planes(self.ctx, self.bwd_planes), "nrw_ctx_set_backward_planes")
-        # backward sweeps rebuild softplus'(a) / softplus''(a) from the stored output planes: with plain-bf16 backward GEMMs
-        # ('mixed') the hi plane alone is enough (tests/test_gpu_precision_policy.py); the strict modes read every plane
-        gate = int(os.environ.get("NRW_BWD_GATE_PLANES", 1 if self.bwd_planes == 1 else 0))
-        if gate:
-            check(self.L.nrw_ctx_set_backward_gate_planes(self.ctx, min(gate, self.n_planes)), "nrw_ctx_set_backward_gate_planes")
         self.flat = None
         self.packed = None
         self.workspace = None
