@@ -234,6 +234,32 @@ NRW_API int nrw_network_backward(nrw_ctx* ctx, const nrw_render_cfg* cfg, const 
                                  const float* d_normals, const float* d_rgb, const float* d_bg_alpha,
                                  const float* d_bg_rgb, float* grad_params, float* grad_a_emb, void* stream);
 
+/* ---- appearance codes of held-out photographs against frozen networks (NeRF-W evaluation; rules in csrc/appearance.cu)
+ * nrw_appearance_prepare runs the appearance-free part of nrw_render_forward for the rays of cfg (o, d, z_vals [R,S],
+ * z_out [R,n_outside] (may be NULL when n_outside = 0), sample_dist [R], inv_s [1], as for the render; cfg's
+ * cos_anneal_ratio, background_rgb and trim_sphere apply, reserved0 is not read) and stores into `cache` (caller-owned,
+ * 256-byte aligned, nrw_appearance_cache_bytes(ctx, R, S, n_outside) bytes) everything of `color` that does not depend on
+ * the appearance code: per sample static_linear_0's pre-activation without the code columns (colour net, and the NeRF's
+ * appearance head), the colour layers' [pts | normal] inputs and the compositing weights of the colours; per ray the
+ * constant rest.  nrw_appearance_forward then writes color [R,3], equal to nrw_render_forward's color for the codes
+ * a_emb [R,n_a] up to the split W [x | a] = W [x | 0] + W_a a; nrw_appearance_backward writes grad_a_emb [R,n_a] for the
+ * upstream g_color [R,3] (per-ray sums in a fixed order: reproducible).  Neither forms a weight gradient or runs the SDF
+ * network, xyz_encoding_final or the NeRF trunk.  The cache holds the networks as packed at the prepare (prepare again
+ * after nrw_pack_weights with new weights); the context remembers each prepared cache by its address, and R is not bounded
+ * by the bound max_rays.  Forward and backward run chunk by chunk through the bound workspace (the backward recomputes its
+ * forward; it needs a bind with backward) and invalidate the forward a render left for its backward, which then
+ * recomputes it.  Status: NRW_ERR_ARG for R <= 0 or a NULL required pointer, NRW_ERR_STATE before bind + pack, for a cache
+ * not prepared on this context or a backward without a backward bind, NRW_ERR_WORKSPACE for a cache smaller than
+ * nrw_appearance_cache_bytes.  nrw_appearance_cache_bytes returns a negative nrw_status for sizes out of range. */
+NRW_API long long nrw_appearance_cache_bytes(const nrw_ctx* ctx, int R, int S, int n_outside);
+NRW_API int nrw_appearance_prepare(nrw_ctx* ctx, const nrw_render_cfg* cfg, const float* o, const float* d,
+                                   const float* z_vals, const float* z_out, const float* sample_dist, const float* inv_s,
+                                   void* cache, long long cache_bytes, void* stream);
+NRW_API int nrw_appearance_forward(nrw_ctx* ctx, const void* cache, const float* a_emb /*[R,n_a]*/, float* color /*[R,3]*/,
+                                   void* stream);
+NRW_API int nrw_appearance_backward(nrw_ctx* ctx, const void* cache, const float* a_emb, const float* g_color /*[R,3]*/,
+                                    float* grad_a_emb /*[R,n_a], written*/, void* stream);
+
 /* ---- octree near/far (tools/prepare_data/generate_voxel.py:311-439) ---------------------- */
 /* octree bytes (breadth-first, one per non-leaf), prefix = exclusive popcount sum (#nodes entries),
  * pyramid int32 [2, level+2].  rays in the SfM frame.  Outputs near,far [R] (already * scale),

@@ -252,6 +252,39 @@ int nrw_network_backward(nrw_ctx* ctx, const nrw_render_cfg* cfg, const nrw_rend
   NRW_GUARD_END
 }
 
+long long nrw_appearance_cache_bytes(const nrw_ctx* ctx, int R, int S, int n_outside) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx && R > 0 && S >= 1 && n_outside >= 0, NRW_ERR_ARG,
+            "appearance_cache_bytes: null context or R=%d S=%d n_outside=%d out of range", R, S, n_outside);
+  return appearance_cache_bytes(*ctx, R, S, n_outside);
+  NRW_GUARD_END
+}
+int nrw_appearance_prepare(nrw_ctx* ctx, const nrw_render_cfg* cfg, const float* o, const float* d, const float* z_vals,
+                           const float* z_out, const float* sample_dist, const float* inv_s, void* cache, long long cache_bytes,
+                           void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx && cfg && o && d && z_vals && sample_dist && inv_s && cache, NRW_ERR_ARG, "appearance_prepare: null argument");
+  NRW_CHECK(cfg->R > 0 && cfg->S >= 1 && cfg->n_outside >= 0, NRW_ERR_ARG, "appearance_prepare: R=%d S=%d n_outside=%d",
+            cfg->R, cfg->S, cfg->n_outside);
+  NRW_CHECK(cfg->n_outside == 0 || z_out, NRW_ERR_ARG, "appearance_prepare: n_outside=%d needs z_out", cfg->n_outside);
+  NRW_CHECK((reinterpret_cast<uintptr_t>(cache) & 255) == 0, NRW_ERR_ARG, "appearance_prepare: cache must be 256B aligned");
+  return appearance_prepare(*ctx, *cfg, o, d, z_vals, z_out, sample_dist, inv_s, cache, cache_bytes, S(stream));
+  NRW_GUARD_END
+}
+int nrw_appearance_forward(nrw_ctx* ctx, const void* cache, const float* a_emb, float* color, void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx && cache && a_emb && color, NRW_ERR_ARG, "appearance_forward: null argument");
+  return appearance_forward(*ctx, cache, a_emb, color, S(stream));
+  NRW_GUARD_END
+}
+int nrw_appearance_backward(nrw_ctx* ctx, const void* cache, const float* a_emb, const float* g_color, float* grad_a_emb,
+                            void* stream) {
+  NRW_GUARD_BEGIN
+  NRW_CHECK(ctx && cache && a_emb && g_color && grad_a_emb, NRW_ERR_ARG, "appearance_backward: null argument");
+  return appearance_backward(*ctx, cache, a_emb, g_color, grad_a_emb, S(stream));
+  NRW_GUARD_END
+}
+
 int nrw_octree_near_far(const uint8_t* octree, const int32_t* prefix, const int32_t* pyramid_host, int level,
                         const float* rays_o, const float* rays_d, int R, const float scene_origin[3], float scale,
                         float* near, float* far, int32_t* pid, int32_t* count, void* stream) {

@@ -365,7 +365,76 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(nrw_render_cfg cfg, 
   if (lane == 0 && d_inv_s) atomicAdd(d_inv_s, dinvs);
 }
 
+// The weights that composite_fwd_kernel applies to the per-sample colours for `color`, from the same ray_forward:
+// w_fg[r,i] (i < S) multiplies rgb[r,i], w_bg[r,i] (i < T, when bg_alpha) multiplies bg_rgb[r,i], and cst[r] collects
+// everything else: background_rgb * (1 - weights_sum), plus the background colours when bg_rgb is given (then w_bg may be
+// NULL: the caller folds a background that does not depend on anything it varies).
+template <int CPL>
+__global__ void __launch_bounds__(128) composite_weights_kernel(nrw_render_cfg cfg, nrw_render_io io,
+                                                                const float* __restrict__ sdf,
+                                                                const float* __restrict__ nrm,
+                                                                const float* __restrict__ bg_alpha,
+                                                                const float* __restrict__ bg_rgb,
+                                                                float* __restrict__ w_fg, float* __restrict__ w_bg,
+                                                                float* __restrict__ cst) {
+  const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (r >= cfg.R) return;
+  const int S = cfg.S, T = cfg.S + cfg.n_outside;
+  RayFwd<CPL> F;
+  ray_forward<CPL>(cfg, io, r, lane, sdf, nrm, bg_alpha, F);
+  float x[CPL], Tm[CPL];
+#pragma unroll
+  for (int k = 0; k < CPL; ++k) x[k] = (lane * CPL + k < T) ? 1.0f - F.A[k] + 1e-7f : 1.0f;
+  ray_excl_cumprod<CPL>(x, Tm, lane);
+  float ws = 0.0f, cb[3] = {0, 0, 0};
+#pragma unroll
+  for (int k = 0; k < CPL; ++k) {
+    const int i = lane * CPL + k;
+    if (i >= T) continue;
+    const float w = F.A[k] * Tm[k];
+    float wb = w;   // weight of bg_rgb[r,i]: w (1 - inside) on the SDF samples, w past them
+    if (i < S) {
+      const float in = F.inside[k];
+      w_fg[(long long)r * S + i] = w * in;
+      ws += w * in;
+      wb = w * (1.0f - in);
+    }
+    if (bg_alpha) {
+      if (w_bg) w_bg[(long long)r * T + i] = wb;
+      if (bg_rgb) {
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) cb[ch] += bg_rgb[((long long)r * T + i) * 3 + ch] * wb;
+      }
+    }
+  }
+  ws = warp_sum(ws);
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) cb[ch] = warp_sum(cb[ch]);
+  if (lane == 0) {
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) cst[r * 3 + ch] = cb[ch] + (cfg.background_rgb ? cfg.background_rgb[ch] * (1.0f - ws) : 0.0f);
+  }
+}
+
 static int pick_cpl(int T) { return T <= 160 ? 5 : (T <= 256 ? 8 : (T <= 512 ? 16 : 40)); }
+
+int composite_weights(const nrw_render_cfg& cfg, const nrw_render_io& io, const float* sdf, const float* nrm,
+                      const float* bg_alpha, const float* bg_rgb, float* w_fg, float* w_bg, float* cst, cudaStream_t s) {
+  const int T = cfg.S + cfg.n_outside;
+  NRW_CHECK(T <= 1280, NRW_ERR_ARG, "composite: T=%d samples per ray exceeds 1280", T);
+  const int grid = cdiv((long long)cfg.R * 32, 128);
+  if (grid == 0) return NRW_OK;
+#define NRW_W(C) composite_weights_kernel<C><<<grid, 128, 0, s>>>(cfg, io, sdf, nrm, bg_alpha, bg_rgb, w_fg, w_bg, cst)
+  switch (pick_cpl(T)) {
+    case 5: NRW_W(5); break;
+    case 8: NRW_W(8); break;
+    case 16: NRW_W(16); break;
+    default: NRW_W(40);
+  }
+#undef NRW_W
+  NRW_LAUNCH_OK();
+  return NRW_OK;
+}
 
 int composite_forward(const nrw_render_cfg& cfg, const nrw_render_io& io, const float* sdf, const float* nrm,
                       const float* rgb, const float* bg_alpha, const float* bg_rgb, float* ge_acc, cudaStream_t s) {

@@ -165,7 +165,7 @@ static GemmDesc mm_desc(int P, Planes A, Planes B, int M, int N, int K, Epi e) {
   g.epi = e;
   return g;
 }
-static int mm(nrw_ctx& c, int P, Planes A, Planes B, int M, int N, int K, Epi e, cudaStream_t s) {
+int mm(nrw_ctx& c, int P, Planes A, Planes B, int M, int N, int K, Epi e, cudaStream_t s) {
   return gemm(c.backend, mm_desc(P, A, B, M, N, K, e), s);
 }
 // dW[layer] += dY^T X   (dY [M, Np], X [M, Kx]); atomically accumulated into the gradient scratch
@@ -300,6 +300,11 @@ int color_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, cons
   NRW_TRY(launch_color_embed(dirs, a, c.n_a, rows_per_src, pts, f.c_nrm, M, P, f.IN1, f.IN2, s));
   { Epi e; e.bias = c.bias(L_CX); e.out_pl = f.IN1; NRW_TRY(mm(c, P, f.FEAT, c.W(L_CX), M, 512, 512, e, s)); }
   { Epi e; e.bias = c.bias(L_CS0); e.act = ACT_RELU; e.out_pl = f.H1; NRW_TRY(mm(c, P, f.IN1, c.W(L_CS0), M, 128, 640, e, s)); }
+  return color_chunk_tail(c, f, M, s);
+}
+
+int color_chunk_tail(nrw_ctx& c, FwdSdfSlot& f, int M, cudaStream_t s) {
+  const int P = c.n_planes;
   { Epi e; e.bias = c.bias(L_CS1); e.act = ACT_RELU; e.out_pl = f.IN2; NRW_TRY(mm(c, P, f.H1, c.W(L_CS1), M, 128, 128, e, s)); }
   { Epi e; e.bias = c.bias(L_CL0); e.act = ACT_RELU; e.out_pl = f.X[1]; NRW_TRY(mm(c, P, f.IN2, c.W(L_CL0), M, 256, 192, e, s)); }
   for (int l = 1; l <= 3; ++l) {
@@ -334,6 +339,11 @@ int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const 
   { Epi e; e.bias = c.bias(L_NF); e.out_pl = f.FEATN; NRW_TRY(mm(c, P, f.NH[8], c.W(L_NF), M, 256, 256, e, s)); }
   // L_NS0 is static_linear_0 of the appearance head, or views_linears.0 without it (the last layer before rgb_linear)
   { Epi e; e.bias = c.bias(L_NS0); e.act = ACT_RELU; e.out_pl = f.AP[1]; NRW_TRY(mm(c, P, f.FEATN, c.W(L_NS0), M, 128, 384, e, s)); }
+  return nerf_rgb_tail(c, f, M, s);
+}
+
+int nerf_rgb_tail(nrw_ctx& c, FwdNerfSlot& f, int M, cudaStream_t s) {
+  const int P = c.n_planes;
   const int last = c.nerf_app ? 4 : 1;
   for (int l = 1; l < last; ++l) {
     Epi e; e.bias = c.bias(L_NS0 + l); e.act = ACT_RELU; e.out_pl = f.AP[l + 1];
@@ -662,31 +672,6 @@ int sample(nrw_ctx& c, const nrw_sampler_cfg& cfg, int R, const float* o, const 
     NRW_TRY(launch_boundary(R, S0, cfg.boundary_samples, near, far, c.gz[cur], z_vals, s));
   } else {
     NRW_CUDA_OK(cudaMemcpyAsync(z_vals, c.gz[cur], (size_t)R * S0 * 4, cudaMemcpyDeviceToDevice, s));
-  }
-  return NRW_OK;
-}
-
-// The chunks of one pass over R rays and the slots that keep their forward.  With k slots for n chunks, chunk i writes
-// slot min(i, k - 1) in the forward (visit j is chunk j), so chunks 0 .. k-2 stay resident and so does the last chunk,
-// the last one written into slot k - 1.  The backward takes chunks 0 .. k-2 from their slots, then the last chunk
-// (still in slot k - 1), then recomputes chunks k-1 .. n-2 into slot k - 1; with k >= n that is chunk order.  Without
-// `cached` the backward recomputes every chunk.
-struct ChunkVisit { int ci, slot; bool resident; };
-static ChunkVisit chunk_visit(int j, int n, int k, bool backward, bool cached) {
-  const int last = (n < k ? n : k) - 1;
-  const int ci = !backward || j < last ? j : j == last ? n - 1 : j - 1;
-  return ChunkVisit{ci, ci < last ? ci : last, backward && cached && (ci == n - 1 || ci < last)};
-}
-
-// Runs chunk(slot, resident, r0, nr, M) on every chunk of a pass in the order of chunk_visit: rays [r0, r0 + nr) of T
-// samples each, M = nr * T rows.
-template <class Slot, class F>
-static int walk_chunks(nrw_ctx& c, std::vector<Slot>& slots, int R, int T, bool backward, bool cached, F&& chunk) {
-  const int rc = c.Mc / T, n = cdiv(R, rc);
-  for (int j = 0; j < n; ++j) {
-    const ChunkVisit v = chunk_visit(j, n, (int)slots.size(), backward, cached);
-    const int r0 = v.ci * rc, nr = (R - r0) < rc ? (R - r0) : rc;
-    NRW_TRY(chunk(slots[v.slot], v.resident, r0, nr, nr * T));
   }
   return NRW_OK;
 }

@@ -1,5 +1,6 @@
 // Orchestration of the per-ray hot path over L2-sized chunks of samples.
 #pragma once
+#include <map>
 #include <vector>
 
 #include "gemm.h"
@@ -24,6 +25,11 @@ struct FwdNerfSlot {
   float *c_density, *c_alpha, *c_rgbbg, *c_dists;
 };
 
+// shape of an appearance cache prepared on this context (nrw_appearance_prepare); its layout follows from it (appearance.cu)
+struct AppCacheDims {
+  int R, S, n_outside;
+};
+
 struct nrw_ctx {
   int n_planes = 2, backend = 0, n_vocab = 0, n_a = 48;
   int bwd_planes = 2;   // planes of the backward GEMMs and of u for their softplus gates: n_planes, or 1 in 'mixed'
@@ -40,6 +46,7 @@ struct nrw_ctx {
   bool bound = false, packed_valid = false;
   const float* params = nullptr;
   int Mc = 0, with_bwd = 0, max_rays = 0, max_T = 0;
+  std::map<const void*, AppCacheDims> app_caches;   // caches prepared on this context, by device address
 
   // 'mixed' on the tensor cores: Q_l (l != 0, 4) and the second-order terms DA2_l are stored as one bf16 plane
   // (gemm_simt takes fp32 side streams only)
@@ -78,6 +85,34 @@ long long workspace_bytes(const nrw_ctx& c, int chunk_rows, int with_bwd, int ma
 int carve_workspace(nrw_ctx& c, void* base, long long bytes, int chunk_rows, int with_bwd, int max_rays,
                     int max_T, int n_slots_sdf, int n_slots_nerf, cudaStream_t s);
 
+// one GEMM D = A B^T through the context's backend with the epilogue e, on P operand planes
+int mm(nrw_ctx& c, int P, Planes A, Planes B, int M, int N, int K, Epi e, cudaStream_t s);
+
+// The chunks of one pass over R rays and the slots that keep their forward.  With k slots for n chunks, chunk i writes
+// slot min(i, k - 1) in the forward (visit j is chunk j), so chunks 0 .. k-2 stay resident and so does the last chunk,
+// the last one written into slot k - 1.  The backward takes chunks 0 .. k-2 from their slots, then the last chunk
+// (still in slot k - 1), then recomputes chunks k-1 .. n-2 into slot k - 1; with k >= n that is chunk order.  Without
+// `cached` the backward recomputes every chunk.
+struct ChunkVisit { int ci, slot; bool resident; };
+inline ChunkVisit chunk_visit(int j, int n, int k, bool backward, bool cached) {
+  const int last = (n < k ? n : k) - 1;
+  const int ci = !backward || j < last ? j : j == last ? n - 1 : j - 1;
+  return ChunkVisit{ci, ci < last ? ci : last, backward && cached && (ci == n - 1 || ci < last)};
+}
+
+// Runs chunk(slot, resident, r0, nr, M) on every chunk of a pass in the order of chunk_visit: rays [r0, r0 + nr) of T
+// samples each, M = nr * T rows.
+template <class Slot, class F>
+int walk_chunks(nrw_ctx& c, std::vector<Slot>& slots, int R, int T, bool backward, bool cached, F&& chunk) {
+  const int rc = c.Mc / T, n = cdiv(R, rc);
+  for (int j = 0; j < n; ++j) {
+    const ChunkVisit v = chunk_visit(j, n, (int)slots.size(), backward, cached);
+    const int r0 = v.ci * rc, nr = (R - r0) < rc ? (R - r0) : rc;
+    NRW_TRY(chunk(slots[v.slot], v.resident, r0, nr, nr * T));
+  }
+  return NRW_OK;
+}
+
 // SDF value (+ normals, + feature planes) for M rows at positions pts [M,3]; results in f.c_sdf / f.c_nrm / f.FEAT
 int sdf_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, bool need_normal, bool need_feat,
                       cudaStream_t s);
@@ -85,6 +120,10 @@ int color_chunk_forward(nrw_ctx& c, FwdSdfSlot& f, int M, const float* pts, cons
                         int rows_per_src, cudaStream_t s);
 int nerf_chunk_forward(nrw_ctx& c, FwdNerfSlot& f, int M, const float* o, const float* d, const float* z,
                        const float* sdist, const float* pts4, const float* a, int T, int rows_per_src, cudaStream_t s);
+// the layers after the code-reading static_linear_0 of each colour branch: f.H1 (with f.IN2's [pts | normal] columns) ->
+// f.c_rgb, and f.AP[1] -> f.c_rgbbg
+int color_chunk_tail(nrw_ctx& c, FwdSdfSlot& f, int M, cudaStream_t s);
+int nerf_rgb_tail(nrw_ctx& c, FwdNerfSlot& f, int M, cudaStream_t s);
 // backward of the three networks for the chunk whose forward slot f holds
 int color_chunk_backward(nrw_ctx& c, const FwdSdfSlot& f, int M, const float* d_rgb, const float* d_nrm_comp,
                          int rows_per_src, float* d_a_rays, int R_chunk, cudaStream_t s, float* d_pts = nullptr);
@@ -124,5 +163,14 @@ int render_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& 
 int network_backward(nrw_ctx& c, const nrw_render_cfg& cfg, const nrw_render_io& io, const float* d_sdf,
                      const float* d_nrm, const float* d_rgb, const float* d_bga, const float* d_bgc, float* grad_params,
                      float* grad_a_emb, cudaStream_t s);
+
+// appearance-code fitting on a cached appearance-free render prefix (appearance.cu, include/nrw.h)
+long long appearance_cache_bytes(const nrw_ctx& c, int R, int S, int n_outside);
+int appearance_prepare(nrw_ctx& c, const nrw_render_cfg& cfg, const float* o, const float* d, const float* z_vals,
+                       const float* z_out, const float* sample_dist, const float* inv_s, void* cache, long long cache_bytes,
+                       cudaStream_t s);
+int appearance_forward(nrw_ctx& c, const void* cache, const float* a_emb, float* color, cudaStream_t s);
+int appearance_backward(nrw_ctx& c, const void* cache, const float* a_emb, const float* g_color, float* grad_a_emb,
+                        cudaStream_t s);
 
 }  // namespace nrw

@@ -60,5 +60,8 @@ int composite_backward(const nrw_render_cfg& cfg, const nrw_render_io& io, const
                        const float* sdf, const float* nrm, const float* rgb, const float* bg_alpha,
                        const float* bg_rgb, float* d_sdf, float* d_nrm, float* d_rgb, float* d_bg_alpha,
                        float* d_bg_rgb, float* d_inv_s, cudaStream_t s);
+// the per-sample weights of `color` (composite.cu composite_weights_kernel) for the appearance cache
+int composite_weights(const nrw_render_cfg& cfg, const nrw_render_io& io, const float* sdf, const float* nrm,
+                      const float* bg_alpha, const float* bg_rgb, float* w_fg, float* w_bg, float* cst, cudaStream_t s);
 
 }  // namespace nrw

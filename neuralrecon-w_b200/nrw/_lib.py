@@ -107,6 +107,11 @@ def lib():
     L.nrw_composite_forward.argtypes = [C.POINTER(RenderCfg), C.POINTER(RenderIO)] + [vp] * 7
     L.nrw_composite_backward.argtypes = [C.POINTER(RenderCfg), C.POINTER(RenderIO), C.POINTER(RenderGrads)] + [vp] * 7
     L.nrw_network_backward.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(RenderIO)] + [vp] * 8
+    L.nrw_appearance_cache_bytes.restype = ll
+    L.nrw_appearance_cache_bytes.argtypes = [vp, i32, i32, i32]
+    L.nrw_appearance_prepare.argtypes = [vp, C.POINTER(RenderCfg)] + [vp] * 7 + [ll, vp]
+    L.nrw_appearance_forward.argtypes = [vp, vp, vp, vp, vp]
+    L.nrw_appearance_backward.argtypes = [vp, vp, vp, vp, vp, vp]
     L.nrw_octree_near_far.argtypes = [vp, vp, vp, i32, vp, vp, i32, C.POINTER(f32), f32, vp, vp, vp, vp, vp]
     L.nrw_octree_hits.argtypes = [vp, vp, vp, i32, vp, vp, i32, C.POINTER(f32), f32, vp, vp, vp, vp, vp]
     L.nrw_octree_build_scratch_bytes.restype = ll
@@ -184,7 +189,8 @@ EXPORTS = ["nrw_last_error", "nrw_version", "nrw_param_count", "nrw_param_table"
            "nrw_reproject_mark", "nrw_raygen_capacity", "nrw_raygen_scratch_bytes", "nrw_raygen_image",
            "nrw_depth_range_scratch_bytes", "nrw_depth_range", "nrw_voxel_cast", "nrw_voxel_lookup",
            "nrw_view_roi_count", "nrw_label_static_count", "nrw_first_hit_scratch_bytes", "nrw_first_hit",
-           "nrw_obs_reproj_error", "nrw_ctx_set_nerf_appearance", "nrw_neuconw_backward", "nrw_nerf_backward"]
+           "nrw_obs_reproj_error", "nrw_ctx_set_nerf_appearance", "nrw_neuconw_backward", "nrw_nerf_backward",
+           "nrw_appearance_cache_bytes", "nrw_appearance_prepare", "nrw_appearance_forward", "nrw_appearance_backward"]
 
 
 def check(status, what=""):

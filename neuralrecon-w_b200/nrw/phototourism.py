@@ -3,7 +3,7 @@
 
     read_scene        read_meta steps 1-4: tsv, images.bin / cameras.bin / points3D.bin, K, c2w, near/far bounds
     RayGenerator      one image -> the reference's cache rows and rgbs (csrc/raygen.cu, rules in its header)
-    PhototourismDataset  the reference's constructor, __len__ and __getitem__ for "train" and "val" / "test_train"
+    PhototourismDataset  the reference's constructor, __len__ and __getitem__ for "train", "val" / "test_train" and "eval"
 
 Images are decoded and LANCZOS-downscaled by PIL on the host (as the reference does) by a small thread pool that runs
 ahead of the device.  Deviations from the reference are listed in INTEGRATION.md.
@@ -298,15 +298,19 @@ class RayGenerator:
 
 
 class PhototourismDataset(torch.utils.data.Dataset):
-    """datasets/phototourism.py::PhototourismDataset for split "train" (use_cache or in-memory generation) and
-    "val" / "test_train" (one image generated on the fly).  "eval", "test" and shared_cache raise NrwError."""
+    """datasets/phototourism.py::PhototourismDataset for split "train" (use_cache or in-memory generation),
+    "val" / "test_train" and "eval" (one image generated on the fly).  "test" and shared_cache raise NrwError.
+
+    "eval" serves the test-split images (img_ids_test) with the reference's keys; its left / right halves are the pixels
+    with column x < w // 2 and the rest, in raster order (INTEGRATION.md: the reference's reshape(-1, 9) of its 12- or
+    13-column rows misaligns them)."""
 
     def __init__(self, root_dir, split="train", img_downscale=1, val_num=1, use_cache=False, cache_paths=["cache"],
                  split_path="", semantic_map_path=None, with_semantics=True, use_voxel=True, scene_origin=None,
                  scene_radius=None, shared_cache=False, shared_rays_base=None, shared_rgbs_base=None, all_rays_shape=None,
                  all_rgbs_shape=None, device=0, sfm_path=None, depth_percent=None, seed=0):
-        if split not in ("train", "val", "test_train"):
-            raise NrwError(f"PhototourismDataset: split {split!r} is not supported (train, val, test_train)")
+        if split not in ("train", "val", "test_train", "eval"):
+            raise NrwError(f"PhototourismDataset: split {split!r} is not supported (train, val, test_train, eval)")
         if shared_cache:
             raise NrwError("PhototourismDataset: shared_cache is not supported")
         if img_downscale < 1:
@@ -350,6 +354,12 @@ class PhototourismDataset(torch.utils.data.Dataset):
                 self.all_rays.append(rows.cpu())
                 self.all_rgbs.append(rgbs.cpu())
             check_voxel_misses(n_miss, len(self.img_ids_train))
+        elif split == "eval":
+            if with_semantics:   # the reference reads every test image's semantic map in its constructor
+                for id_ in self.img_ids_test:
+                    path = os.path.join(root_dir, f"{semantic_map_path}/{self.image_paths[id_].split('.')[0]}.npz")
+                    if not os.path.isfile(path):
+                        raise NrwError(f"semantic map {path} not found")
         else:
             self.val_id = self.img_ids_train[0]
 
@@ -358,6 +368,8 @@ class PhototourismDataset(torch.utils.data.Dataset):
             return len(self.all_rays)
         if self.split == "test_train":
             return self.N_images_train
+        if self.split == "eval":
+            return self.N_images_test
         return self.val_num
 
     def __getitem__(self, idx):
@@ -369,6 +381,8 @@ class PhototourismDataset(torch.utils.data.Dataset):
             else:
                 sample["rays"] = torch.cat((self.all_rays[idx, :8], self.all_rays[idx, 9:12]), dim=-1)
             return sample
+        if self.split == "eval":
+            return self._eval_sample(self.img_ids_test[idx])
         id_ = self.val_id if self.split == "val" else self.img_ids_train[idx]
         sample = {"c2w": torch.FloatTensor(self.poses_dict[id_])}
         img, sem = self.gen.decode(id_)
@@ -384,6 +398,20 @@ class PhototourismDataset(torch.utils.data.Dataset):
         sample["img_wh"] = torch.LongTensor([w, h])
         sample["K"] = self.Ks[id_]
         return sample
+
+    def _eval_sample(self, id_):
+        """datasets/phototourism.py:726-748: the image's rays, split into the left (x < w // 2) and right halves"""
+        img, sem = self.gen.decode(id_)
+        rows, rgbs, _ = self.gen.run(id_, img, sem)
+        h, w = int(img.shape[0]), int(img.shape[1])
+        rows, rgbs = rows.cpu(), rgbs.cpu()
+        rays, ts = rows[:, :8], rows[:, 8].long()
+        left = (torch.arange(h * w) % w) < w // 2
+        return {"rays": rays, "ts": ts, "rgbs": rgbs,
+                "rays_train": rays[left], "ts_train": ts[left], "rgbs_train_gt": rgbs[left],
+                "rays_eval": rays[~left], "ts_eval": ts[~left], "rgbs_eval_gt": rgbs[~left],
+                "extrinsic": torch.FloatTensor(self.poses_dict[id_]), "intrinsic": self.Ks[id_],
+                "img_wh": torch.LongTensor([w, h]), "image_name": self.image_paths[id_]}
 
 
 def check_voxel_misses(n_miss, n_images):
